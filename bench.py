@@ -44,9 +44,6 @@ import torch  # noqa: E402
 from valley_b200 import synthetic as syn  # noqa: E402
 
 GFLOP_PER_FRAME = {-2: 155.29, -1: 162.02}     # BASELINE.md section 3
-# committed ncu --set full captures of decode_step_kernel, per (model, batch): dram bytes per launch (profiles/)
-NCU_DECODE = {("valley2-7b", 1): "prof_mega_r02_7b_b1_summary.csv", ("valley-13b", 4): "prof_mega_r02_13b_b4_summary.csv",
-              ("valley-13b", 1): "prof_mega_r02_13b_b1_summary.csv"}
 
 
 def prompt_len(n_frames):
@@ -58,7 +55,8 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sust=d.get("bf16_tflops_sustained", d["bf16_tflops"]), src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, src="fallback")
+    # NVIDIA's H100 SXM data sheet (700 W part): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 -- an upper bound, not a measured rate
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sust=989.0, src="H100 SXM data sheet")
 
 
 def usable_cpus():
@@ -105,25 +103,6 @@ def cpu_has_bf16_units():
         return False
 
 
-def ncu_traffic(spec_name, B):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of decode_step_kernel from the committed ncu --set full capture of
-    THIS (model, batch) -- None when no capture of that configuration is committed."""
-    name = NCU_DECODE.get((spec_name, B))
-    if not name:
-        return None, None
-    try:
-        import csv
-        rows = list(csv.reader(open(os.path.join(ROOT, "profiles", name))))
-        hdr, units, row = rows[0], rows[1], rows[2]
-        tot = 0.0
-        for k in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-            i = hdr.index(k)
-            tot += float(row[i]) * {"Gbyte": 1e9, "Mbyte": 1e6, "Kbyte": 1e3, "byte": 1.0}.get(units[i], 1.0)
-        return tot, "profiles/" + name
-    except Exception:
-        return None, None
-
-
 def decode_bytes_per_step(spec, B, S):
     """Algorithmic HBM bytes of one decode step (SURVEY 8d): every weight once (bf16) + KV read + KV write."""
     H, I, V, L = spec.hidden_size, spec.intermediate_size, spec.vocab_size, spec.num_hidden_layers
@@ -133,7 +112,7 @@ def decode_bytes_per_step(spec, B, S):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -268,7 +247,7 @@ class CpuReferenceArm:
 
 
 def gpu_eager_reference(spec, B, n_frames, n_new, decode_tokens=16):
-    """SURVEY 8d "reference GPU path": the same oracle (the ATen ops the reference's HF modules run, eager, bf16) on the B200 itself.
+    """SURVEY 8d "reference GPU path": the same oracle (the ATen ops the reference's HF modules run, eager, bf16) on the same GPU.
     Not a target and not the product -- it says how much of the speed-up is the GPU and how much is this repo."""
     from oracle import valley_oracle as O
     dev, dt = "cuda", torch.bfloat16
@@ -316,7 +295,7 @@ def gpu_eager_reference(spec, B, n_frames, n_new, decode_tokens=16):
     del w
     torch.cuda.empty_cache()
     total = ms_vit + ms_prefill + (n_new - 1) * ms_dec
-    return {"what": "oracle (eager torch ops, bf16) on the same B200", "tokens_per_s": B * n_new / (total / 1e3), "vit_frames_per_s": B * n_frames / (ms_vit / 1e3),
+    return {"what": "oracle (eager torch ops, bf16) on the same GPU", "tokens_per_s": B * n_new / (total / 1e3), "vit_frames_per_s": B * n_frames / (ms_vit / 1e3),
             "prefill_ms": ms_prefill, "decode_ms_per_step": ms_dec, "decode_tokens_per_s": B * 1e3 / ms_dec}
 
 
@@ -334,6 +313,9 @@ def main():
     ap.add_argument("--no-7b", action="store_true", help="skip the extra valley2-7b B=1 figures (BASELINE config 2)")
     ap.add_argument("--vit-sweep", action="store_true", help="also time ViT encode over F (BASELINE config 5); N > 1: strong scaling, F fixed")
     ap.add_argument("--gpu-eager-baseline", action="store_true", help="also time the oracle as eager torch-CUDA ops on the GPU (SURVEY 8d)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (the generated token ids) as DIR/<name>.npy "
+                         "(float64); inputs and weights are seeded, so two builds can be compared output for output")
     a = ap.parse_args()
     spec = syn.SPECS[a.model]
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
@@ -490,12 +472,17 @@ def main():
         clk.start()
     ms_step, launches, toks = timed(step_device, a.steps, max(a.warmup, 3))
     clocks = clk.stop() if rank == 0 else None
+    if a.dump_outputs:
+        import numpy as np
+        os.makedirs(a.dump_outputs, exist_ok=True)
+        name = "tokens" if world == 1 else f"tokens_rank{rank}"          # [videos of this rank, new tokens], exact in float64
+        np.save(os.path.join(a.dump_outputs, name + ".npy"), toks.detach().cpu().numpy().astype(np.float64))
     ms_e2e, _, toks_e2e = timed(step_e2e, a.steps, 1)
 
     # ---- the two halves of the metric, timed separately on the device ----
     def vit_only(F, mdl=None):
         px = syn.make_pixels(1, F, 1, dtype=torch.float16)[0].cuda()
-        return timed(lambda: (mdl or model).encode_frames(px), max(a.steps, 5), 3, mdl)[0]
+        return timed(lambda: (mdl or model).encode_frames(px), a.steps, 3, mdl)[0]
     F_req = B * T
     ms_vit_req = vit_only(F_req)
     ms_vit8 = vit_only(8) if F_req != 8 else ms_vit_req
@@ -596,12 +583,11 @@ def main():
             ms7, l7, _ = timed(lambda: m7.generate(input_ids=ids7, images=px7, max_new_tokens=128, eos_token_id=None)[:, S7:], 3, 2, m7)
             d7, smid7, p7, _, k7 = llm_only(m7, s7, 1, 8, 128)
             b7 = decode_bytes_per_step(s7, 1, smid7)
-            tr7, src7 = ncu_traffic("valley2-7b", 1)
             cfg2 = {"workload": "valley2-7b bf16: 1 video x 8 frames, prompt S=333, greedy 128 new tokens [BASELINE config 2]",
                     "tokens_per_s": 128 / (ms7 / 1e3), "ms_per_request": ms7, "gpu_launches_per_request": int(l7 / 3),
                     "decode_ms_per_token": d7, "decode_tokens_per_s": 1e3 / d7, "prefill_ms": p7,
                     "roofline": {"kernel": k7, "bound": "hbm", "achieved": b7 / (d7 / 1e3) / 1e9, "peak": peaks()["hbm"], "unit": "GB/s",
-                                 "frac": b7 / (d7 / 1e3) / 1e9 / peaks()["hbm"], "algorithmic_bytes_per_launch": b7, "traffic": tr7, "traffic_source": src7}}
+                                 "frac": b7 / (d7 / 1e3) / 1e9 / peaks()["hbm"], "algorithmic_bytes_per_launch": b7}}
             del m7
             torch.cuda.empty_cache()
 
@@ -617,7 +603,6 @@ def main():
     fps_req = F_req / (ms_vit_req / 1e3)
     fps8 = 8 / (ms_vit8 / 1e3)
     gf = GFLOP_PER_FRAME.get(spec.mm_vision_select_layer, 155.29) if spec.vit_layers == 24 else None
-    traffic, traffic_src = ncu_traffic(a.model, B)
     line = {
         "metric": metric, "value": value, "unit": "tokens/s", "n_gpus": a.gpus, "steps": a.steps, "warmup": max(a.warmup, 3), "ms_per_step": ms_step,
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16",
@@ -632,12 +617,11 @@ def main():
         "vit_frames_per_s": world * fps_req, "vit_frames_per_encode": F_req, "vit_ms_per_encode": ms_vit_req,
         "vit_frames_per_s_at_8_frames": world * fps8, "prefill_ms": ms_prefill, "vit_sweep_frames_per_s": sweep,
         "roofline": {"kernel": f"{dec_kernel} (one persistent cooperative launch = one decode step of all {B} sequences: every weight streamed once through a TMA ring"
-                               + ("; tcgen05 consumer" if "umma" in dec_kernel else "") + ")",
+                               + ")",
                      "bound": "hbm", "achieved": dec_gbs, "peak": pk["hbm"], "unit": "GB/s", "frac": dec_gbs / pk["hbm"], "peak_source": pk["src"],
-                     "algorithmic_bytes_per_launch": dec_bytes, "traffic": traffic, "traffic_source": traffic_src,
-                     "note": "peak = measured read+write copy bandwidth; a read-only stream on this part reaches 7.2-7.5 TB/s (tools/membw.cu)"},
+                     "algorithmic_bytes_per_launch": dec_bytes},
         "roofline_vit": None if gf is None else {
-            "kernel": f"ViT-L/14 encode (gemm_tc_kernel + vit_attention_pp_kernel), F={F_req} (the request's frames in one encode)", "bound": "tensor",
+            "kernel": f"ViT-L/14 encode (gemm_tc_kernel + vit_attention_kernel), F={F_req} (the request's frames in one encode)", "bound": "tensor",
             "achieved": fps_req * gf / 1e3, "peak": pk["tf_burst"], "unit": "TFLOP/s", "frac": fps_req * gf / 1e3 / pk["tf_burst"],
             "frac_at_8_frames": fps8 * gf / 1e3 / pk["tf_burst"], "gflop_per_frame": gf, "peak_source": pk["src"],
             "sweep_frac_of_sustained": {k: v * gf / 1e3 / pk["tf_sust"] for k, v in sweep.items()}},

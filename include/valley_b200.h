@@ -1,4 +1,4 @@
-/* valley_b200.h -- C ABI of libvalley_b200.so: the B200-native (sm_100a) implementation of Valley's
+/* valley_b200.h -- C ABI of libvalley_b200.so: the H100-native (sm_90a) implementation of Valley's
  * multimodal forward hot path (CLIP ViT-L/14 encode -> temporal pool + mm_projector -> LLaMA decoder
  * with KV cache -> greedy token).
  *
@@ -210,10 +210,9 @@ int vly_generate(vly_ctx* ctx, vly_kv* kv, const int64_t* first_tokens_dev, int 
 int vly_kernel_launch_count(vly_ctx* ctx, int64_t* out);   /* kernels launched by this ctx so far */
 int vly_num_sms(vly_ctx* ctx, int* out);
 
-/* in-kernel cycle counters of the last decode step / ViT attention launch, filled only when the process runs with VLY_MEGA_DBG=1 /
- * VLY_ATTN_DBG=1 (tools/bench_decode.py, tools/bench_vit.py): copies n int64 values to host_out; returns 0, -1 (never enabled) or -2. */
+/* in-kernel cycle counters of the last decode step, filled only when the process runs with VLY_MEGA_DBG=1
+ * (tools/bench_decode.py): copies n int64 values to host_out; returns 0, -1 (never enabled) or -2. */
 int vly_debug_mega_counters(long long* host_out, int n);
-int vly_debug_attn_counters(long long* host_out, int n);
 /* internal: lets the host-only translation units (host_splice.cpp, host_preprocess.cpp) set the thread-local error message */
 void vly_set_error_(const char* message);
 

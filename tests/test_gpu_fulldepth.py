@@ -4,7 +4,7 @@ The tiny / one-layer tests prove the kernels; bf16 error grows with depth (every
 stream), so the stated bar is checked here at depth:  rel-Frobenius against the fp32 oracle <= 2e-2, or -- where 32-40 layers of
 bf16 rounding exceed that for ANY bf16 implementation -- no worse than 1.5x the error of the same oracle run as eager torch-bf16
 ops (which is what a user of the reference runs on a GPU); greedy ids exact wherever the oracle's top-1/top-2 margin exceeds 2x
-the max logit error.  Measured numbers are printed (pytest -s) and recorded in DESIGN.md.  Checked on
+the max logit error.  Measured numbers are printed (pytest -s) and recorded in BASELINE.md.  Checked on
 
     (a) ViT-L/14, all 24 layers loaded, ``select_layer=-2`` (23 executed) and ``-1`` (24), F = 8 frames       [configs 2-5]
     (b) valley2-7b  (Llama-2-7B shape, 32 layers), B = 1, 8 frames: prefill + 8 teacher-forced decode steps    [config 2]
@@ -38,9 +38,30 @@ def _true_fp32():
     torch.cuda.empty_cache()
 
 
+class _Fp32View(dict):
+    """bf16 tensors on the GPU, handed out as fp32 one access at a time: the fp32 oracle sees exactly the values of a bf16
+    checkpoint without 4 bytes per parameter staying resident (the 13B model's 52 GB of fp32 weights do not fit an 80 GB GPU
+    next to the packed model)."""
+
+    def __getitem__(self, k):
+        return dict.__getitem__(self, k).float()
+
+    def get(self, k, default=None):
+        return self[k] if k in self else default
+
+    def items(self):
+        return ((k, self[k]) for k in self.keys())
+
+    def values(self):
+        return (self[k] for k in self.keys())
+
+    def bf16(self):
+        return {k: dict.__getitem__(self, k) for k in self.keys()}
+
+
 def _gpu_weights(spec, seed=0, **kw):
-    """fp32 tensors on the GPU holding bf16-representable values (what a bf16 checkpoint contains); one pass, no host copy"""
-    return {k: v.bfloat16().float() for k, v in syn.iter_state_dict(spec, seed, device="cuda", **kw)}
+    """the weights as bf16 tensors on the GPU (what a bf16 checkpoint contains), read as fp32; one pass, no host copy"""
+    return _Fp32View((k, v.bfloat16()) for k, v in syn.iter_state_dict(spec, seed, device="cuda", **kw))
 
 
 def _build(spec, sd):
@@ -60,7 +81,7 @@ def test_vit_l14_full_depth_vs_fp32_oracle(sel):
     got = m._vit_encode(px.half(), sel)                                   # callers send fp16 pixels (valley_model.py:430)
     with torch.no_grad():
         ref = O.vit_hidden_state(sd, px.half().float(), sel, num_layers=24)
-        ref_bf = O.vit_hidden_state({k: v.bfloat16() for k, v in sd.items()}, px.half().bfloat16(), sel, num_layers=24)
+        ref_bf = O.vit_hidden_state(sd.bf16(), px.half().bfloat16(), sel, num_layers=24)
     e, eb = Hh.rel_fro(got, ref), Hh.rel_fro(ref_bf, ref)
     print(f"ViT-L/14 select {sel}: rel-Fro ours {e:.3e}, torch-bf16 {eb:.3e}, absmax ref {ref.abs().max().item():.2f}")
     assert torch.isfinite(got.float()).all()
@@ -79,7 +100,7 @@ def _llm_parity(spec, B, T, n_steps, seed=0):
     with torch.no_grad():
         r_tok, r_log = O.greedy_generate(sd, cfg, tok, ids.cuda(), px.float().cuda(), n_steps, return_logits=True)
         # the SAME oracle as eager torch-bf16 ops, teacher-forced with the fp32 oracle's tokens: the error any bf16 run has at this depth
-        sd_bf = {k: v.bfloat16() for k, v in sd.items()}
+        sd_bf = sd.bf16()
         cache_bf, bf_logs = O.KVCache(spec.num_hidden_layers), []
         for i in range(n_steps):
             cur = ids.cuda() if i == 0 else r_tok[:, i - 1:i]
@@ -143,8 +164,8 @@ def test_valley2_7b_full_depth_prefill_and_decode_vs_fp32_oracle():
 
 def test_valley_13b_b4_full_depth_prefill_and_decode_vs_fp32_oracle():
     """BASELINE config 3 (the metric's model): valley-13b (40 layers), 4 videos x 8 frames; the decode steps run
-    decode_step_umma_kernel<4> (tcgen05 consumer), the prefill the CTA-pair GEMMs at M = 1332."""
+    decode_step_kernel<4> (tensor-core consumer), the prefill the 256-wide GEMM tiles at M = 1332."""
     free = torch.cuda.mem_get_info()[0]
-    if free < 120e9:
-        pytest.skip(f"needs ~110 GB of device memory for the fp32 oracle weights + the packed model (free: {free / 1e9:.0f} GB)")
+    if free < 64e9:
+        pytest.skip(f"needs ~60 GB of device memory for the bf16 oracle weights + the packed model (free: {free / 1e9:.0f} GB)")
     _llm_parity(syn.VALLEY_13B, B=4, T=8, n_steps=9)

@@ -679,7 +679,7 @@ def test_cache_capacity_is_enforced():
 def test_production_shapes_one_layer(spec_name, B):
     """One decoder layer at the real 7B / 13B widths (H 4096/5120, I 11008/13824, 32/40 heads, V 32008): prefill logits and
     6 teacher-forced decode steps vs the oracle -- covers the K-tail slices of the CUDA-core (B = 1) and tensor-core (B > 1)
-    decode consumers and the 256-wide / CTA-pair GEMM tilings."""
+    decode consumers and the 128- / 256-wide GEMM tilings."""
     spec = syn.SPECS[spec_name]
     sd = Hh.bf16_weights(spec, 2)
     m = Hh.build_model(spec, sd)
@@ -741,11 +741,17 @@ def _decode_parity(spec_name, B, n=8, seed=0, len_a=20, len_b=11):
 
 
 @pytest.mark.parametrize("B", [2, 3, 4])
-def test_tcgen05_decode_consumer_full_and_tail_stages(B):
-    """decode_step_umma_kernel (B = 2..4, K multiples of 512): tiny-umma has intermediate_size 3584 = one 2560-column stage + a 1024-column
-    tail stage per work unit of down_proj (two sub-phases on one staged activation block); prefill + 8 teacher-forced steps +
-    free-running ids vs the oracle.  B = 1 on the same model runs decode_step_kernel<1> (the reference point)."""
+def test_tensor_core_decode_consumer_batches(B):
+    """decode_step_kernel<2 / 4> (the m16n8k16 tensor-core consumer for B = 2..4) on tiny-umma (intermediate_size 3584):
+    prefill + 8 teacher-forced steps + free-running ids vs the oracle."""
     _decode_parity("tiny-umma", B)
+
+
+def test_tensor_core_decode_consumer_ragged_k():
+    """intermediate_size = 3776 = 59 panels of 64 columns (Llama-2-7B: 11008 = 172): down_proj's K is not a multiple of the ring
+    stage width, so the last stage of every work unit is a short one.  B = 2 and B = 4."""
+    for B in (2, 4):
+        _decode_parity("tiny-umma-ragged", B)
 
 
 @pytest.mark.parametrize("len_a,len_b", [(230, 120), (400, 250)])
@@ -755,26 +761,3 @@ def test_decode_attention_multi_pass_items_at_production_head_count(len_a, len_b
     pass, up to 5 % of the items in a second round) -- the regime the headline request spends its second half in.  Prefill logits,
     8 teacher-forced decode steps and free-running ids vs the oracle."""
     _decode_parity("shape-13b-1l", 4, len_a=len_a, len_b=len_b)
-
-
-def _decode_parity_subprocess(env, calls):
-    import subprocess
-    import sys
-    code = ("import sys; sys.path.insert(0, %r); sys.path.insert(0, %r); import test_gpu_parity as t; print('ERR', %s)"
-            % (os.path.dirname(__file__), os.path.dirname(os.path.dirname(__file__)), ", ".join("t._decode_parity(%r, %d)" % c for c in calls)))
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600, env=dict(os.environ, **env))
-    assert r.returncode == 0 and "ERR" in r.stdout, r.stdout[-1500:] + r.stderr[-1500:]
-
-
-def test_tcgen05_decode_consumer_ragged_k():
-    """intermediate_size = 3776 = 59 panels of 64 columns (Llama-2-7B: 11008 = 172): the K walk is rounded up to whole 512-column
-    groups and the panels beyond the real K are out of bounds in both tensor maps (zero fill, no memory read).  Not the default for
-    such shapes (measured slower than the mma.sync consumer on Llama-2-7B), so it is forced with VLY_DECODE_UMMA=2."""
-    _decode_parity_subprocess({"VLY_DECODE_UMMA": "2"}, [("tiny-umma-ragged", 2), ("tiny-umma-ragged", 4)])
-
-
-def test_tcgen05_decode_consumer_restaged_sub_phases():
-    """The same with VLY_UMMA_XC=512: the activation block holds 512 columns, so down_proj (K = 3584) is walked in SEVEN sub-phases
-    with the block re-staged behind a CTA-local barrier and the accumulators resident in TMEM in between -- the mechanism the 13B
-    model uses for K = 13824 (3 pieces).  The switch is read once per process, hence the subprocess."""
-    _decode_parity_subprocess({"VLY_UMMA_XC": "512"}, [("tiny-umma", 4), ("tiny-umma", 2)])

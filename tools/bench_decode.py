@@ -35,10 +35,11 @@ print(f"{a.model} B={a.batch}: {best:.3f} ms/token  {a.batch / best * 1e3:.1f} t
       f"env V1={os.environ.get('VLY_DECODE_V1')} NO_PDL={os.environ.get('VLY_NO_PDL')}  tokens[0,:6]={out[0,:6].tolist()}")
 if os.environ.get("VLY_MEGA_DBG"):
     import ctypes as C
-    buf = (C.c_longlong * (148 * 32))()
-    rc = m._lib.vly_debug_mega_counters(buf, 148 * 32)
+    n_sm = torch.cuda.get_device_properties(0).multi_processor_count
+    buf = (C.c_longlong * (n_sm * 32))()
+    rc = m._lib.vly_debug_mega_counters(buf, n_sm * 32)
     import numpy as np
-    arr = np.array(buf[:]).reshape(148, 32)
+    arr = np.array(buf[:]).reshape(n_sm, 32)
     names = ["grid sync", "stage x", "weight loop", "attention"]
     print("last step, cycle breakdown (mean over CTAs | min | max), SM clock cycles (~1.9 GHz):")
     for i, nme in enumerate(names):

@@ -20,14 +20,4 @@ for F in a.frames:
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(); out = m.encode_frames(px); e1.record(); torch.cuda.synchronize()
         best = min(best, e0.elapsed_time(e1))
-    print(f"ViT-L/14 F={F}: {best:.3f} ms  {F / best * 1e3:.0f} frames/s  {F / best * 1e3 * 155.29 / 1e3:.0f} TFLOP/s  nan={int(torch.isnan(out.float()).sum())} env V1={os.environ.get('VLY_VIT_ATTN_V1')}")
-if os.environ.get("VLY_ATTN_DBG"):
-    import ctypes as C, numpy as np
-    buf = (C.c_longlong * (148 * 16))()
-    m._lib.vly_debug_attn_counters(buf, 148 * 16)
-    arr = np.array(buf[:]).reshape(148, 16)
-    names = ["T0 total", "T0 wait r_free", "T0 wait q_full", "T0 wait k_full", "T0 wait k_done", "T0 wait p_full", "T0 exec MMA issue", "T0 exec Q-TMA issue",
-             "WG-A total", "WG-A wait q/s_full", "WG-A bar(max xchg)", "WG-A wait o_full", "WG-B total", "WG-B wait q/s_full", "WG-B bar", "WG-B wait o_full"]
-    print("last attention launch, cycles (mean over CTAs):")
-    for i, n in enumerate(names):
-        print(f"  {n:22s} {arr[:, i].mean():10.0f}")
+    print(f"ViT-L/14 F={F}: {best:.3f} ms  {F / best * 1e3:.0f} frames/s  {F / best * 1e3 * 155.29 / 1e3:.0f} TFLOP/s  nan={int(torch.isnan(out.float()).sum())}")

@@ -1,7 +1,7 @@
 """ctypes binding of libvalley_b200.so (the C ABI in include/valley_b200.h).
 
 There is no fallback: if the shared library is missing, import fails loudly with the build
-command; if no sm_100 GPU is visible, ``vly_create`` fails with the library's own message.
+command; if no sm_90 GPU is visible, ``vly_create`` fails with the library's own message.
 """
 from __future__ import annotations
 
@@ -85,7 +85,6 @@ SIGNATURES = {
     "vly_kernel_launch_count": (_i, [_vp, _p(_i64)]),
     "vly_num_sms": (_i, [_vp, _p(_i)]),
     "vly_debug_mega_counters": (_i, [_vp, _i]),
-    "vly_debug_attn_counters": (_i, [_vp, _i]),
     "vly_set_error_": (None, [C.c_char_p]),
     "vly_test_gemm": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp]),
     "vly_test_vit_attention": (_i, [_vp, _vp, _i, _vp, _vp]),
@@ -102,7 +101,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} not found. Build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). valley_b200 has no CPU or PyTorch fallback.")
+            "(nvcc, sm_90a). valley_b200 has no CPU or PyTorch fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in SIGNATURES.items():
         if not hasattr(lib, name) and os.environ.get("VLY_LIB_PATH"):

@@ -21,7 +21,6 @@
 #include "simt_kernels.cuh"
 #include "decode_kernels.cuh"
 #include "decode_mega.cuh"
-#include "decode_umma.cuh"
 #include "preprocess.cuh"
 #include "pooling_kernels.cuh"
 
@@ -41,7 +40,7 @@ static int fail(int code, const char* fmt, ...) {
   return code;
 }
 extern "C" const char* vly_last_error(void) { return g_err; }
-extern "C" const char* vly_version(void) { return "valley_b200 0.1 (sm_100a)"; }
+extern "C" const char* vly_version(void) { return "valley_b200 0.1 (sm_90a)"; }
 
 #define CK(expr)                                                                                       \
   do {                                                                                                 \
@@ -93,7 +92,7 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
 
 struct vly_ctx {
   vly_config cfg;
-  int num_sms = 148;
+  int num_sms = 0;
   PFN_encodeTiled encode = nullptr;
   std::mutex mu;
   std::map<std::string, Staged> staged;
@@ -164,9 +163,6 @@ struct vly_kv {
   int nsplit = 1, gemv_grid = 0;
   int stage_bytes = 0;                 // ring slot of the persistent decode kernel: max over its phases (pick_phase_geometry)
   int n_grid_syncs = 0;                // grid barriers per decode launch
-  bool umma = false;                   // B = 2..4 on the tcgen05 consumer (decode_umma.cuh)
-  int umma_x_cols = 0;                 // columns of the swizzled activation block of that kernel
-  void* d_tmaps = nullptr;             // CUtensorMap[] of the weight matrices (one per phase geometry)
   PhaseDesc* d_phases = nullptr;
   int n_phases = 0;
   unsigned int* grid_counter = nullptr;
@@ -283,101 +279,17 @@ static cudaError_t launch_ex(Kern kern, dim3 grid, dim3 block, size_t smem, cuda
 // ------------------------------------------------------------------------------------------------
 // GEMM launcher
 // ------------------------------------------------------------------------------------------------
-// TMA-store epilogue (gemm_tc.cuh, TEPI): bf16 row-major outputs whose rows the TMA unit can address (16-byte aligned base and pitch)
-template <int EPI>
-static bool gemm_tepi_ok(const GemmParams& p) {
-  static const int env = getenv("VLY_GEMM_TEPI") ? atoi(getenv("VLY_GEMM_TEPI")) : 1;
-  if (!env) return false;
-  // (measured: it pays where the epilogue, not the main loop, sets the pace -- K <= 2048: ViT F = 64 10.24 -> 9.47 ms; with the
-  //  LLaMA widths, K = 4096 .. 13824, the 5-stage ring it needs costs more than the stores save: 13B prefill 46.6 -> 47.4 ms)
-  // ... except the residual epilogue of a LONG K = 4096 GEMM with few column tiles (the ViT's fc2 at >= 48 frames: 9.59 -> 9.20 ms at
-  // 64 frames), where the row-wise residual loads + stores still rival the main loop
-  if (p.K > 2048 && env < 2 && !(EPI == EPI_BIAS_RES_STATS && p.K <= 4096 && p.M >= 12000)) return false;
-  // The GEMM that also pushes its tiles to the peers (fused all-gather) keeps the register-store epilogue: that combination is the one
-  // verified bit-identical to NCCL on 2 AND 8 GPUs.  With the staged epilogue it was bit-identical on 2 GPUs, but the one 8-GPU
-  // run taken with it reported a mismatch (profiles/bench_r02_n8_tepi_gather_mismatch.json).  Suspected (DESIGN 6): the residual-box
-  // refill in the staged epilogue is issued before the ld.shared of that box are known to have retired; behind 7 peers' NVLink stores
-  // they can still be queued when the TMA write lands.  To be fixed and re-verified on 8 GPUs before this is switched on.
-  if (p.n_peers > 0 && env < 2) return false;
-  if (!(EPI == EPI_BIAS || EPI == EPI_LN_BIAS || EPI == EPI_LN_BIAS_GELU || EPI == EPI_BIAS_RES_STATS || EPI == EPI_RMS_SWIGLU)) return false;
-  if ((p.ldo & 7) || (reinterpret_cast<uintptr_t>(p.out) & 15)) return false;
-  if (EPI == EPI_BIAS_RES_STATS && ((p.ldr & 7) || (reinterpret_cast<uintptr_t>(p.residual) & 15))) return false;
-  return true;
-}
-
 template <int BN, int EPI>
 static int launch_gemm_t(vly_ctx* c, const bf16* A, long long lda, const bf16* W, long long ldw, GemmParams p, cudaStream_t st) {
   using Cfg = GemmCfg<BN>;
-  constexpr bool kTepiMode = (EPI == EPI_BIAS || EPI == EPI_LN_BIAS || EPI == EPI_LN_BIAS_GELU || EPI == EPI_BIAS_RES_STATS || EPI == EPI_RMS_SWIGLU);
-  CUtensorMap ta, tb, to, tr;
+  CUtensorMap ta, tb;
   TRY(make_tmap_2d(c, &ta, A, p.K, p.M, lda * 2, 64, 128));
   TRY(make_tmap_2d(c, &tb, W, p.K, p.N, ldw * 2, 64, BN));
-  to = ta; tr = ta;                                        // (placeholders when the epilogue stores from registers)
-  const bool tepi = gemm_tepi_ok<EPI>(p);
-  if (tepi) {
-    const int n_out = (EPI == EPI_RMS_SWIGLU) ? p.N / 2 : p.N;
-    TRY(make_tmap_2d(c, &to, p.out, n_out, p.M, p.ldo * 2, 64, 32));
-    if (EPI == EPI_BIAS_RES_STATS) TRY(make_tmap_2d(c, &tr, p.residual, p.N, p.M, p.ldr * 2, 64, 32));
-  }
   p.num_m_tiles = cdiv(p.M, 128);
   p.num_n_tiles = cdiv(p.N, BN);
   const int tiles = p.num_m_tiles * p.num_n_tiles;
-  // CTA-pair mode (cta_group::2, 256 x 256 tile per pair): halves the B traffic per SM (64 instead of 96 B/cycle/SM of
-  // L2->SM operand traffic).  Used when there is enough work to fill the pairs; VLY_GEMM_CG2=0/1 overrides.
-  if constexpr (BN == 256) {
-    static const int cg2_env = getenv("VLY_GEMM_CG2") ? atoi(getenv("VLY_GEMM_CG2")) : -1;
-    const int pairs = c->num_sms / 2;
-    const int pair_tiles = cdiv(p.num_m_tiles, 2) * p.num_n_tiles;
-    // (measured: pairs win from one full wave of pair tiles on -- ViT, 32 frames: 5.23 -> 5.10 ms; below that -- 16 frames, 68 tiles of
-    //  the N = 1024 GEMMs -- the single-CTA tiles spread better: 3.05 vs 3.09 ms)
-    //  An odd, small number of 128-row tiles wastes the pair's second half (M = 333: 3 tiles -> 4): those wait for two full waves.
-    const bool small_odd = (p.num_m_tiles & 1) && p.num_m_tiles < 7;
-    const bool use_cg2 = cg2_env >= 0 ? (cg2_env == 1) : (pair_tiles >= (small_odd ? 2 : 1) * pairs);
-    if (use_cg2) {
-      CUtensorMap tb2;
-      TRY(make_tmap_2d(c, &tb2, W, p.K, p.N, ldw * 2, 64, BN / 2));
-      cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3(2 * (pair_tiles < pairs ? pair_tiles : pairs));
-      cfg.blockDim = dim3(Cfg::THREADS);
-      cfg.stream = st;
-      cudaLaunchAttribute attr[2];
-      attr[0].id = cudaLaunchAttributeClusterDimension;
-      attr[0].val.clusterDim.x = 2;
-      attr[0].val.clusterDim.y = 1;
-      attr[0].val.clusterDim.z = 1;
-      attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      attr[1].val.programmaticStreamSerializationAllowed = 1;
-      cfg.attrs = attr;
-      cfg.numAttrs = pdl_enabled() ? 2 : 1;
-      if constexpr (kTepiMode) {
-        if (tepi) {
-          constexpr int smem = gemm_smem_bytes<BN, true>();
-          TRY(ensure_smem_attr(c->cfg.device, gemm_tc_kernel<BN, EPI, true, true>, smem));
-          cfg.dynamicSmemBytes = smem;
-          CK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, EPI, true, true>, ta, tb2, to, tr, p));
-          c->launches++;
-          return VLY_OK;
-        }
-      }
-      TRY(ensure_smem_attr(c->cfg.device, gemm_tc_kernel<BN, EPI, true, false>, Cfg::SMEM_BYTES));
-      cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-      CK(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, EPI, true, false>, ta, tb2, to, tr, p));
-      c->launches++;
-      return VLY_OK;
-    }
-  }
-  const int grid = tiles < c->num_sms ? tiles : c->num_sms;
-  if constexpr (kTepiMode && BN == 128) {
-    if (tepi) {
-      constexpr int smem = gemm_smem_bytes<BN, true>();
-      TRY(ensure_smem_attr(c->cfg.device, gemm_tc_kernel<BN, EPI, false, true>, smem));
-      CK(launch_ex(gemm_tc_kernel<BN, EPI, false, true>, dim3(grid), dim3(Cfg::THREADS), smem, st, true, ta, tb, to, tr, p));
-      c->launches++;
-      return VLY_OK;
-    }
-  }
-  TRY(ensure_smem_attr(c->cfg.device, gemm_tc_kernel<BN, EPI, false, false>, Cfg::SMEM_BYTES));
-  CK(launch_ex(gemm_tc_kernel<BN, EPI, false, false>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, true, ta, tb, to, tr, p));
+  TRY(ensure_smem_attr(c->cfg.device, gemm_tc_kernel<BN, EPI>, Cfg::SMEM_BYTES));
+  CK(launch_ex(gemm_tc_kernel<BN, EPI>, dim3(tiles), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, true, ta, tb, p));
   c->launches++;
   return VLY_OK;
 }
@@ -388,29 +300,17 @@ static int launch_gemm(vly_ctx* c, int bn, const bf16* A, long long lda, const b
   return launch_gemm_t<128, EPI>(c, A, lda, W, ldw, p, st);
 }
 static inline int pick_bn(int N) { return (N % 256 == 0) ? 256 : 128; }
-// Tile width by wave efficiency: a persistent launch runs ceil(tiles / SMs) rounds, so what counts is how full the last round
-// is.  M = 2056 (8 frames), N = 3072: 128 x 256 tiles -> 204 tiles = 2 rounds at 69 %; 128 x 128 -> 408 tiles = 3 half-size rounds
-// at 92 %.  256-wide tiles are kept when they are within 5 % (better operand reuse per SM).  M-dependent, so callers that
-// exchange row statistics compute it ONCE per (N, M) and pass it around.
+// Tile width by wave efficiency: one CTA per SM at a time, so a launch runs ceil(tiles / SMs) rounds and what counts is how full
+// the last round is.  M = 2056 (8 frames), N = 3072 on 132 SMs: 128 x 256 tiles -> 204 tiles = 2 rounds at 77 %; 128 x 128 -> 408
+// tiles = 4 half-size rounds at 77 %.  256-wide tiles are kept unless the narrow ones fill the rounds > 5 % better (256 columns
+// halve the A traffic per output).  M-dependent, so callers that exchange row statistics compute it ONCE per (N, M) and pass it
+// around.  VLY_GEMM_BN=128|256 forces a width.
 static inline int pick_bn_m(const vly_ctx* c, int N, int M) {
   if (N % 256 != 0) return 128;
-  static const int env_bn = getenv("VLY_GEMM_BN") ? atoi(getenv("VLY_GEMM_BN")) : 0;      // 128 / 256: force (A/B measurements)
+  static const int env_bn = getenv("VLY_GEMM_BN") ? atoi(getenv("VLY_GEMM_BN")) : 0;
   if (env_bn == 128 || env_bn == 256) return env_bn;
   const long long t256 = (long long)cdiv(M, 128) * (N / 256), t128 = 2 * t256;
   if (t256 >= 3LL * c->num_sms) return 256;            // many rounds: the last one matters little, operand reuse matters more
-  {
-    // CTA pairs (256 x 256 tiles, launch_gemm_t) sustain ~1.5x the rate of single 128 x 128 tiles (ncu, LLaMA-13B prefill: 1.22 vs
-    // 0.82 PFLOP/s), so a reasonably full pair launch beats a perfectly full 128-wide one: M = 1332, N = 5120 -- 120 pair tiles on 74
-    // pairs, 11 of 12 row tiles real = 0.74 -- took 3.2 ms off the 13B prefill (47.9 -> 44.7).  Below ~0.7 (8 ViT frames: 0.69) the
-    // narrow tiles stay.
-    const int mt = cdiv(M, 128), pairs = c->num_sms / 2;
-    const long long pt = (long long)cdiv(mt, 2) * (N / 256);
-    const bool small_odd = (mt & 1) && mt < 7;
-    if (pt >= (small_odd ? 2 : 1) * pairs) {
-      const double e_pair = (double)pt / ((double)cdiv(pt, pairs) * pairs) * ((double)mt / (2.0 * cdiv(mt, 2)));
-      if (e_pair >= 0.70) return 256;
-    }
-  }
   const double e256 = (double)t256 / ((double)cdiv(t256, c->num_sms) * c->num_sms);
   const double e128 = (double)t128 / ((double)cdiv(t128, c->num_sms) * c->num_sms);
   return (e128 > e256 * 1.05) ? 128 : 256;
@@ -515,7 +415,7 @@ extern "C" int vly_create(const vly_config* cfg, vly_ctx** out) {
   CK(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10) return fail(VLY_ERR_CUDA, "vly_create: device is sm_%d%d; this library is built for sm_100a only", prop.major, prop.minor);
+  if (prop.major != 9) return fail(VLY_ERR_CUDA, "vly_create: device is sm_%d%d; this library is built for sm_90a only", prop.major, prop.minor);
   if (cfg->hidden_size % 128 || cfg->hidden_size / cfg->num_attention_heads != 128)
     return fail(VLY_ERR_INVALID, "vly_create: head_dim must be 128 (hidden %d, heads %d)", cfg->hidden_size, cfg->num_attention_heads);
   if (cfg->intermediate_size % 64) return fail(VLY_ERR_INVALID, "vly_create: intermediate_size must be a multiple of 64");
@@ -831,47 +731,23 @@ extern "C" int vly_finalize_weights(vly_ctx* c) {
 // ------------------------------------------------------------------------------------------------
 // ViT encode
 // ------------------------------------------------------------------------------------------------
-static long long* g_attn_dbg = nullptr;
-extern "C" int vly_debug_attn_counters(long long* host_out, int n) {
-  if (!g_attn_dbg) return -1;
-  return cudaMemcpy(host_out, g_attn_dbg, (size_t)n * 8, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -2;
-}
 static int launch_vit_attention(vly_ctx* c, const bf16* qkv, int F, bf16* out, cudaStream_t st) {
   const vly_config& g = c->cfg;
   const int D = g.vit_hidden, tokens = (g.vit_image / g.vit_patch) * (g.vit_image / g.vit_patch) + 1;
-  if (tokens != 257) return fail(VLY_ERR_INVALID, "vit attention kernel is specialised for 257 tokens (got %d)", tokens);
-  TRY(ensure_smem_attr(c->cfg.device, vit_attention_kernel, VitAttnCfg::SMEM_BYTES));
-  CUtensorMap tq, tkv;
-  TRY(make_tmap_2d(c, &tq, qkv, 3 * D, (uint64_t)F * tokens, (uint64_t)3 * D * 2, 64, 128));
-  TRY(make_tmap_2d(c, &tkv, qkv, 3 * D, (uint64_t)F * tokens, (uint64_t)3 * D * 2, 64, 136));
+  using C = FlashCfg<64>;
+  TRY(ensure_smem_attr(c->cfg.device, vit_attention_kernel, C::SMEM_BYTES));
+  CUtensorMap tq;
+  TRY(make_tmap_2d(c, &tq, qkv, 3 * D, (uint64_t)F * tokens, (uint64_t)3 * D * 2, 64, 64));
   VitAttnParams p;
   p.F = F;
   p.tokens = tokens;
   p.heads = g.vit_heads;
   p.D = D;
   p.ctx = out;
-  p.qkv = qkv;
   p.scale_log2e = 0.125f * 1.4426950408889634f;
-  {
-    static long long* dbg = nullptr;
-    if (getenv("VLY_ATTN_DBG") && !dbg) { CK(cudaMalloc((void**)&dbg, 148 * 16 * 8)); CK(cudaMemset(dbg, 0, 148 * 16 * 8)); }
-    p.dbg = dbg;
-    g_attn_dbg = dbg;
-  }
-  const int items = F * g.vit_heads;
-  const int grid = items < c->num_sms ? items : c->num_sms;
-  static const bool v1 = getenv("VLY_VIT_ATTN_V1") != nullptr;
-  if (!v1) {
-    TRY(ensure_smem_attr(c->cfg.device, vit_attention_pp_kernel, VitAttnPPCfg::SMEM_BYTES));
-    CUtensorMap tx;
-    TRY(make_tmap_2d(c, &tx, qkv, 3 * D, (uint64_t)F * tokens, (uint64_t)3 * D * 2, 64, 1, /*swizzle128=*/false));   // single rows, read linearly
-    CK(launch_ex(vit_attention_pp_kernel, dim3(grid), dim3(VitAttnPPCfg::THREADS), VitAttnPPCfg::SMEM_BYTES, st, true, tq, tx, p));
-    c->launches++;
-    return VLY_OK;
-  }
-  vit_attention_kernel<<<grid, VitAttnCfg::THREADS, VitAttnCfg::SMEM_BYTES, st>>>(tq, tkv, p);
+  const int grid = F * g.vit_heads * cdiv(tokens, 64);
+  CK(launch_ex(vit_attention_kernel, dim3(grid), dim3(C::THREADS), C::SMEM_BYTES, st, true, tq, p));
   c->launches++;
-  CKL();
   return VLY_OK;
 }
 
@@ -919,7 +795,7 @@ static int vit_encode_impl(vly_ctx* c, const void* pixels, int pixel_dtype, int 
     const char* px = (const char*)pixels + (size_t)f0 * 3 * IMG * IMG * px_elem;
     bf16* x = (bf16*)out_dev + (size_t)f0 * tokens * D;
     bf16* col = (bf16*)c->w_col.p;
-    const int blocks = 148 * 8;
+    const int blocks = c->num_sms * 8;
     if (pixel_dtype == VLY_F32) im2col_kernel<float><<<blocks, 256, 0, st>>>((const float*)px, col, fc, IMG, P, c->kpad);
     else if (pixel_dtype == VLY_BF16) im2col_kernel<bf16><<<blocks, 256, 0, st>>>((const bf16*)px, col, fc, IMG, P, c->kpad);
     else if (pixel_dtype == VLY_F16) im2col_kernel<__half><<<blocks, 256, 0, st>>>((const __half*)px, col, fc, IMG, P, c->kpad);
@@ -1157,7 +1033,7 @@ static int pool_project_after(vly_ctx* c, const bf16* feats, int n_videos, int T
       TRY(launch_gemm<EPI_BIAS>(c, pick_bn_m(c, H, p.M), feats + (size_t)v * T * tokens * D, D, c->proj_w, D, p, st));
     }
     if (!tr) {
-      temporal_max_kernel<<<148 * 2, 256, 0, st>>>(P, vis, T, tokens, H);
+      temporal_max_kernel<<<c->num_sms * 2, 256, 0, st>>>(P, vis, T, tokens, H);
       c->launches++;
       CKL();
       continue;
@@ -1165,7 +1041,7 @@ static int pool_project_after(vly_ctx* c, const bf16* feats, int n_videos, int T
     bf16 *Xp = (bf16*)c->w_xp.p, *KV = (bf16*)c->w_dkv.p, *Q = (bf16*)c->w_dq.p, *att = (bf16*)c->w_datt.p;
     bf16 *X1 = (bf16*)c->w_dx1.p, *F1 = (bf16*)c->w_df1.p, *X2 = (bf16*)c->w_dx2.p;
     const bf16* Xlast = Xp + (size_t)(T - 1) * NP * H;          // rows of the last frame: the only queries that are used (:130)
-    delta_add_pos_kernel<<<148 * 2, 256, 0, st>>>(P, w.pos, Xp, T, tokens, H);
+    delta_add_pos_kernel<<<c->num_sms * 2, 256, 0, st>>>(P, w.pos, Xp, T, tokens, H);
     c->launches++;
     GemmParams p = {};
     p.M = T * NP; p.N = 2 * H; p.K = H; p.out = KV; p.ldo = 2 * H; p.bias = w.in_b + H;          // k | v rows of in_proj
@@ -1183,13 +1059,13 @@ static int pool_project_after(vly_ctx* c, const bf16* feats, int n_videos, int T
     p = {};
     p.M = NP; p.N = w.ffn; p.K = H; p.out = F1; p.ldo = w.ffn; p.bias = w.l1_b;
     TRY(launch_gemm<EPI_BIAS>(c, pick_bn_m(c, p.N, p.M), X1, H, w.l1_w, H, p, st));
-    relu_inplace_kernel<<<148, 256, 0, st>>>(F1, (long long)NP * w.ffn / 8);
+    relu_inplace_kernel<<<c->num_sms, 256, 0, st>>>(F1, (long long)NP * w.ffn / 8);
     c->launches++;
     p = {};
     p.M = NP; p.N = H; p.K = w.ffn; p.out = X2; p.ldo = H; p.bias = w.l2_b; p.residual = X1; p.ldr = H;
     TRY(launch_gemm<EPI_BIAS_RES_STATS>(c, pick_bn_m(c, p.N, p.M), F1, w.ffn, w.l2_w, w.ffn, p, st));
     layernorm_rows_kernel<<<NP, 256, 0, st>>>(X2, w.n2_g, w.n2_b, X2, H, 1e-5f);
-    delta_finish_kernel<<<148 * 2, 256, 0, st>>>(P, X2, vis, T, tokens, H);
+    delta_finish_kernel<<<c->num_sms * 2, 256, 0, st>>>(P, X2, vis, T, tokens, H);
     c->launches += 2;
     CKL();
   }
@@ -1213,10 +1089,10 @@ extern "C" int vly_pool_project(vly_ctx* c, const void* feats, int n_videos, int
     if (!c->pool_U) return fail(VLY_ERR_STATE, "vly_pool_project: model.pooling_layer.weight not loaded");
     TRY(ensure(c->w_score, (size_t)n_videos * T * 4));
     importance_score_kernel<<<dim3(T, n_videos), 256, 0, st>>>((const bf16*)feats, c->pool_U, (float*)c->w_score.p, T, tokens, D);
-    weighted_pool_kernel<<<148 * 4, 256, 0, st>>>((const bf16*)feats, (const float*)c->w_score.p, (bf16*)c->w_pool.p, n_videos, T, tokens, D);
+    weighted_pool_kernel<<<c->num_sms * 4, 256, 0, st>>>((const bf16*)feats, (const float*)c->w_score.p, (bf16*)c->w_pool.p, n_videos, T, tokens, D);
     c->launches++;
   } else {
-    temporal_pool_kernel<<<148 * 4, 256, 0, st>>>((const bf16*)feats, (bf16*)c->w_pool.p, n_videos, T, tokens, D);
+    temporal_pool_kernel<<<c->num_sms * 4, 256, 0, st>>>((const bf16*)feats, (bf16*)c->w_pool.p, n_videos, T, tokens, D);
   }
   c->launches++;
   CKL();
@@ -1255,10 +1131,10 @@ static void mega_smem_layout(const vly_config& g, int bmax, size_t* x_bytes, siz
 }
 static const size_t kMegaSmem = 226 * 1024;
 
-// Ring geometry of one weight phase of the persistent decode kernel: rows per work unit and columns per stage.  Measured with
-// tools/ringbw.cu (the producer's access pattern without consumers, profiles/ringbw_r02.log):
-//   * what streams fastest is ~110-125 KB of bulk copies outstanding per SM (7.3-7.4 TB/s); 64 KB: 6.2-7.1, 190 KB: 6.7-7.0;
-//   * a bulk copy should be >= 4 KB: 8 rows x 2.5 KB stream at 5.9 TB/s where 4 rows x 5 KB reach 7.3;
+// Ring geometry of one weight phase of the persistent decode kernel: rows per work unit and columns per stage.  The rules:
+//   * HBM streams best with a bounded number of bytes of bulk copies outstanding per SM (~100 KB): fewer leave it idle, more
+//     only lengthen the queues;
+//   * a bulk copy should be a few KB (>= 3-4 KB): many small row copies stream slower than fewer large ones;
 //   * the consumers need a few hundred cycles to hand a landed stage back, which takes that stage out of flight: a ring of 3
 //     large stages loses more to this than one of 5 smaller stages, so the target is a stage of 1/5 of the ring budget
 //     (but 16-48 KB), cut so that K divides into EQUAL stages (no short tail stage);
@@ -1271,8 +1147,8 @@ static void pick_phase_geometry(int bmax, size_t ring_budget, int N, int K, int 
   const int pad = tc ? MegaCfg::PAD_TC : 0, gran = tc ? 64 : 8;
   static const int env_kb = getenv("VLY_MEGA_STAGE_KB") ? atoi(getenv("VLY_MEGA_STAGE_KB")) : 0;
   static const int env_rows = getenv("VLY_MEGA_ROWS") ? atoi(getenv("VLY_MEGA_ROWS")) : 0;
-  // measured (same-box A/B of the real step, profiles/decode_ab_r02.txt): CUDA-core path -- 4 slots of 32-41 KB beat 3 (more
-  // bytes in flight) and 6 (the grid barriers queue behind the extra prefetch traffic); tensor-core path -- 8 rows x ~2048 columns
+  // stage size: CUDA-core path 4 slots of ~41 KB (fewer, larger slots put more bytes in flight; more slots make the grid barriers
+  // queue behind the extra prefetch traffic); tensor-core path 8 rows x ~2048 columns
   size_t target = env_kb > 0 ? (size_t)env_kb * 1024 : (tc ? 33 * 1024 + 512 : 41 * 1024);
   if (target > ring_budget / 2) target = ring_budget / 2;
   if (target < 8 * 1024) target = 8 * 1024;
@@ -1324,7 +1200,7 @@ extern "C" int vly_kv_create(vly_ctx* c, int batch, int max_seq, vly_kv** out) {
   CK(cudaEventCreateWithFlags(&kv->len_event, cudaEventDisableTiming));
   kv->d_step = kv->d_len + 1;
   CK(cudaMemset(kv->d_len, 0, 8));
-  // (8 rows tall, rows >= batch stay zero: the tcgen05 decode consumer stages these buffers as 8-row tensor-TMA boxes)
+  // (at least 8 rows, rows >= batch stay zero)
   const size_t act_rows = batch < 8 ? 8 : batch;
   CK(cudaMalloc((void**)&kv->x, act_rows * H * 2));
   CK(cudaMalloc((void**)&kv->q, act_rows * H * 2));
@@ -1352,138 +1228,7 @@ extern "C" int vly_kv_create(vly_ctx* c, int batch, int max_seq, vly_kv** out) {
   }
   CK(cudaMalloc((void**)&kv->key_bits, (size_t)batch * kv->mask_words() * 4));
   CK(cudaMemset(kv->key_bits, 0xff, (size_t)batch * kv->mask_words() * 4));
-  // ---- tcgen05 consumer for B = 2..4 (decode_umma.cuh): needs H a multiple of 512, I of 64, and the activation block + ring in 227 KB ----
-  {
-    static const int env_umma = getenv("VLY_DECODE_UMMA") ? atoi(getenv("VLY_DECODE_UMMA")) : 1;
-    static const int env_xc = getenv("VLY_UMMA_XC") ? atoi(getenv("VLY_UMMA_XC")) : 5120;      // (tests shrink it to force sub-phases)
-    const int bmax = batch <= 1 ? 1 : (batch <= 2 ? 2 : 4);
-    const int xcap = env_xc < H ? H : env_xc;
-    // (I not a multiple of 512 -- Llama-2-7B's 11008 -- works through zero-filled out-of-bounds panels but measured slower than the
-    //  mma.sync consumer there: 3.82 vs 3.58 ms/step at B = 4, three activation re-stagings for down_proj; VLY_DECODE_UMMA=2 forces it)
-    kv->umma = env_umma && bmax > 1 && batch <= 4 && decode_mode() == 2 && (H % 512 == 0) && (I % 512 == 0 || (env_umma >= 2 && I % 64 == 0)) &&
-               H <= 5120 && xcap % 512 == 0 &&
-               cdiv(cdiv(H, UmmaCfg::ROWS), c->num_sms) <= UmmaCfg::ACC_SLOTS;
-    if (kv->umma) {
-      // stage width: the largest multiple of 512 columns <= 2560 that divides K
-      auto kc_of = [](int K) {
-        for (int kc = 2560; kc >= 512; kc -= 512)
-          if (K % kc == 0) return kc;
-        return 512;
-      };
-      std::vector<PhaseDesc> ph;
-      std::vector<CUtensorMap> maps;
-      int err = VLY_OK;
-      auto add_map = [&](const bf16* W, int N, int K, int kc) -> int {       // -> index
-        CUtensorMap m;
-        cuuint64_t dims[3] = {64, (cuuint64_t)N, (cuuint64_t)(K / 64)};
-        cuuint64_t strides[2] = {(cuuint64_t)K * 2, 128};
-        cuuint32_t box[3] = {64, (cuuint32_t)UmmaCfg::ROWS, (cuuint32_t)(kc / 64)};
-        cuuint32_t es[3] = {1, 1, 1};
-        CUresult r = c->encode(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<bf16*>(W), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) err = fail(VLY_ERR_CUDA, "cuTensorMapEncodeTiled(decode weights, N=%d K=%d kc=%d) failed: %d", N, K, kc, (int)r);
-        maps.push_back(m);
-        return (int)maps.size() - 1;
-      };
-      static const int env_oob = getenv("VLY_UMMA_XOOB") ? atoi(getenv("VLY_UMMA_XOOB")) : 1;
-      auto add_xmap = [&](const bf16* X, int K, int x_cols) -> int {
-        CUtensorMap m;
-        // rows >= batch of the 8-row box lie outside the tensor: the TMA unit fills them with zeros without reading memory
-        cuuint64_t dims[3] = {64, (cuuint64_t)(env_oob ? batch : 8), (cuuint64_t)(K / 64)};
-        cuuint64_t strides[2] = {(cuuint64_t)K * 2, 128};
-        cuuint32_t box[3] = {64, 8, (cuuint32_t)(x_cols / 64)};
-        cuuint32_t es[3] = {1, 1, 1};
-        CUresult r = c->encode(&m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<bf16*>(X), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) err = fail(VLY_ERR_CUDA, "cuTensorMapEncodeTiled(decode activations, K=%d box %d) failed: %d", K, x_cols, (int)r);
-        maps.push_back(m);
-        return (int)maps.size() - 1;
-      };
-      std::vector<int> map_of;       // phase -> map index (-1: none)
-      std::vector<int> xmap_of;      // phase -> activation map index (-1: none)
-      int x_cols_max = 0, stage_max = 0, n_sync = 1;
-      // one weight matrix = one or more (sub-)phases: pieces of <= xcap columns (each staged once), a piece = full stages of kc
-      // columns plus, if kc does not divide it, ONE shorter tail stage per unit that re-uses the staged block.  K is walked in whole
-      // 512-column MMA groups: when 512 does not divide it (Llama-2-7B's down_proj, K = 11008) the last group's missing 64-column
-      // panels lie outside BOTH tensor maps (dims use the real K) and the TMA unit zero-fills them without reading memory
-      auto add_matrix = [&](PhaseDesc d, const bf16* W) {
-        const int K_real = d.K, K = cdiv(d.K, 512) * 512;
-        d.ldx = K_real; d.rows = UmmaCfg::ROWS;
-        int k0 = 0;
-        while (k0 < K) {
-          const int piece = (K - k0) < xcap ? (K - k0) : xcap;
-          int kc = kc_of(piece);
-          if (kc < 1536 && kc != piece) kc = piece < 2560 ? (piece / 512) * 512 : 2560;      // only small divisors: full stages + one tail stage
-          const int main_cols = (piece / kc) * kc, tail_cols = piece - main_cols;
-          const bool last_piece = (k0 + piece == K);
-          PhaseDesc q = d;
-          q.k_off = k0; q.K = main_cols; q.kc = kc; q.x_cols = piece; q.x_panel0 = 0;
-          q.flags = (k0 == 0 ? PHF_FIRST : 0);
-          if (tail_cols == 0) q.flags |= last_piece ? PHF_LAST : PHF_LOCAL_SYNC;
-          else q.flags |= PHF_NO_SYNC;
-          ph.push_back(q);
-          map_of.push_back(add_map(W, d.N, K_real, kc));
-          xmap_of.push_back(add_xmap(d.x_in, K_real, piece));
-          if (tail_cols > 0) {
-            PhaseDesc t = d;
-            t.k_off = k0 + main_cols; t.K = tail_cols; t.kc = tail_cols; t.x_cols = 0; t.x_panel0 = main_cols / 64;
-            t.flags = last_piece ? PHF_LAST : PHF_LOCAL_SYNC;
-            ph.push_back(t);
-            map_of.push_back(add_map(W, d.N, K_real, tail_cols));
-            xmap_of.push_back(-1);
-          }
-          if (piece > x_cols_max) x_cols_max = piece;
-          if (UmmaCfg::ROWS * kc * 2 > stage_max) stage_max = UmmaCfg::ROWS * kc * 2;
-          if (last_piece) ++n_sync;
-          k0 += piece;
-        }
-      };
-      for (int l = 0; l < L; ++l) {
-        const LlamaLayerW& w = c->layers[l];
-        PhaseDesc d = {};
-        d.layer = l; d.kcache = kv->k_layer(l); d.vcache = kv->v_layer(l);
-        d.type = PH_QKV; d.N = 3 * H; d.K = H; d.W = w.wqkv; d.x_in = kv->x; d.out = kv->q; add_matrix(d, w.wqkv);
-        d.type = PH_ATTN; d.N = 0; d.K = 0; d.W = nullptr; d.x_in = nullptr; d.out = kv->attn; ph.push_back(d); map_of.push_back(-1); xmap_of.push_back(-1); ++n_sync;
-        d.type = PH_OPROJ; d.N = H; d.K = H; d.W = w.wo; d.x_in = kv->attn; d.out = kv->x; add_matrix(d, w.wo);
-        d.type = PH_GATEUP; d.N = 2 * I; d.K = H; d.W = w.wgu; d.x_in = kv->x; d.out = kv->hb; add_matrix(d, w.wgu);
-        d.type = PH_DOWN; d.N = H; d.K = I; d.W = w.wdown; d.x_in = kv->hb; d.out = kv->x; add_matrix(d, w.wdown);
-      }
-      {
-        PhaseDesc d = {};
-        d.type = PH_LOGITS; d.N = V; d.K = H; d.W = c->lm_head; d.x_in = kv->x; d.out = nullptr; add_matrix(d, c->lm_head);
-      }
-      if (err != VLY_OK) return err;
-      static const int env_if = getenv("VLY_MEGA_INFLIGHT_KB") ? atoi(getenv("VLY_MEGA_INFLIGHT_KB")) : 100;
-      for (PhaseDesc& q : ph) {
-        if (q.type == PH_ATTN) continue;
-        const int sb = UmmaCfg::ROWS * q.kc * 2;
-        q.inflight = (env_if * 1024 + sb / 2) / sb;
-        if (q.inflight < 2) q.inflight = 2;
-      }
-      CK(cudaMalloc(&kv->d_tmaps, maps.size() * sizeof(CUtensorMap)));
-      CK(cudaMemcpy(kv->d_tmaps, maps.data(), maps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
-      for (size_t i = 0; i < ph.size(); ++i)
-      {
-        ph[i].tmap = map_of[i] >= 0 ? (const void*)((const CUtensorMap*)kv->d_tmaps + map_of[i]) : nullptr;
-        ph[i].xmap = xmap_of[i] >= 0 ? (const void*)((const CUtensorMap*)kv->d_tmaps + xmap_of[i]) : nullptr;
-      }
-      kv->umma_x_cols = x_cols_max;
-      kv->stage_bytes = stage_max;
-      kv->n_grid_syncs = n_sync;
-      kv->n_phases = (int)ph.size();
-      if (getenv("VLY_MEGA_DBG")) {
-        fprintf(stderr, "[vly] decode (tcgen05 consumer): B=%d activation block %d columns (%d KB), stage %d B, %d phases (%d grid barriers);", batch,
-                x_cols_max, x_cols_max / 64, stage_max, kv->n_phases, n_sync);
-        for (int i = 0; i < 9 && i < (int)ph.size(); ++i)
-          if (ph[i].type != PH_ATTN)
-            fprintf(stderr, " [type%d N=%d k=%d+%d kc=%d stage_x=%d flags=%d]", ph[i].type, ph[i].N, ph[i].k_off, ph[i].K, ph[i].kc, ph[i].x_cols, ph[i].flags);
-        fprintf(stderr, "\n");
-      }
-      CK(cudaMalloc((void**)&kv->d_phases, ph.size() * sizeof(PhaseDesc)));
-      CK(cudaMemcpy(kv->d_phases, ph.data(), ph.size() * sizeof(PhaseDesc), cudaMemcpyHostToDevice));
-    }
-  }
-  if (!kv->umma) {  // phase table of the persistent decode-step kernel: execution order of one step
+  {  // phase table of the persistent decode-step kernel: execution order of one step
     std::vector<PhaseDesc> ph;
     const int bmax = batch <= 1 ? 1 : (batch <= 2 ? 2 : 4);
     const int pad = bmax > 1 ? MegaCfg::PAD_TC : 0;
@@ -1543,7 +1288,7 @@ extern "C" int vly_kv_create(vly_ctx* c, int batch, int max_seq, vly_kv** out) {
 extern "C" int vly_kv_decode_kernel(vly_kv* kv, char* name, int cap) {
   if (!kv || !name || cap <= 0) return fail(VLY_ERR_INVALID, "vly_kv_decode_kernel: bad argument");
   const int bmax = kv->B <= 1 ? 1 : (kv->B <= 2 ? 2 : 4);
-  if (decode_mode() == 2 && kv->B <= 4) snprintf(name, (size_t)cap, "%s<%d>", kv->umma ? "decode_step_umma_kernel" : "decode_step_kernel", bmax);
+  if (decode_mode() == 2 && kv->B <= 4) snprintf(name, (size_t)cap, "decode_step_kernel<%d>", bmax);
   else snprintf(name, (size_t)cap, "%s", decode_mode() == 0 ? "per-op decode kernels (generation 1)" : "per-op TMA-ring decode kernels");
   return VLY_OK;
 }
@@ -1555,7 +1300,7 @@ extern "C" void vly_kv_destroy(vly_kv* kv) {
   if (kv->graph_n) cudaGraphExecDestroy(kv->graph_n);
   if (kv->h_len) cudaFreeHost(kv->h_len);
   if (kv->len_event) cudaEventDestroy(kv->len_event);
-  void* ps[] = {kv->d_tmaps, kv->d_sample, kv->key_bits, kv->dbg, kv->d_phases, kv->cache, kv->d_len, kv->x, kv->q, kv->attn, kv->hb, kv->part_o, kv->part_ml, kv->counters, kv->part_val, kv->part_idx, kv->logits, kv->cur_tokens, kv->gen_tokens};
+  void* ps[] = {kv->d_sample, kv->key_bits, kv->dbg, kv->d_phases, kv->cache, kv->d_len, kv->x, kv->q, kv->attn, kv->hb, kv->part_o, kv->part_ml, kv->counters, kv->part_val, kv->part_idx, kv->logits, kv->cur_tokens, kv->gen_tokens};
   for (void* p : ps)
     if (p) cudaFree(p);
   delete kv;
@@ -1770,17 +1515,18 @@ static int enqueue_decode_step(vly_ctx* c, vly_kv* kv, int b0, int nb, bool bump
 static int launch_prefill_attention(vly_ctx* c, vly_kv* kv, const bf16* qbuf, int B, int S, int past, int layer, bf16* out, cudaStream_t st) {
   const vly_config& g = c->cfg;
   const int H = g.hidden_size, nH = g.num_attention_heads;
-  TRY(ensure_smem_attr(c->cfg.device, llama_prefill_attention_kernel, PrefillAttnCfg::SMEM_BYTES));
+  using C = FlashCfg<128>;
+  TRY(ensure_smem_attr(c->cfg.device, llama_prefill_attention_kernel, C::SMEM_BYTES));
   CUtensorMap tq, tk, tv;
-  TRY(make_tmap_2d(c, &tq, qbuf, H, (uint64_t)B * S, (uint64_t)H * 2, 64, 128));
-  TRY(make_tmap_3d(c, &tk, kv->k_layer(layer), 128, kv->Smax, (uint64_t)B * nH, 256, (uint64_t)kv->Smax * 256, 64, 128));
-  TRY(make_tmap_3d(c, &tv, kv->v_layer(layer), 128, kv->Smax, (uint64_t)B * nH, 256, (uint64_t)kv->Smax * 256, 64, 128));
+  TRY(make_tmap_2d(c, &tq, qbuf, H, (uint64_t)B * S, (uint64_t)H * 2, 64, 64));
+  TRY(make_tmap_3d(c, &tk, kv->k_layer(layer), 128, kv->Smax, (uint64_t)B * nH, 256, (uint64_t)kv->Smax * 256, 64, 64));
+  TRY(make_tmap_3d(c, &tv, kv->v_layer(layer), 128, kv->Smax, (uint64_t)B * nH, 256, (uint64_t)kv->Smax * 256, 64, 64));
   PrefillAttnParams p;
   p.B = B; p.S = S; p.past = past; p.nH = nH; p.H = H; p.Smax = kv->Smax; p.ctx = out;
   p.scale_log2e = 0.08838834764831845f * 1.4426950408889634f;
   p.key_bits = kv->masked ? kv->key_bits : nullptr; p.mask_words = kv->mask_words();
-  const int n_qt = cdiv(S, 128);
-  CK(launch_ex(llama_prefill_attention_kernel, dim3(B * nH * n_qt), dim3(PrefillAttnCfg::THREADS), PrefillAttnCfg::SMEM_BYTES, st, true, tq, tk, tv, p));
+  const int n_qt = cdiv(S, 64);
+  CK(launch_ex(llama_prefill_attention_kernel, dim3(B * nH * n_qt), dim3(C::THREADS), C::SMEM_BYTES, st, true, tq, tk, tv, p));
   c->launches++;
   return VLY_OK;
 }
@@ -1904,35 +1650,6 @@ static int launch_decode_mega(vly_ctx* c, vly_kv* kv, cudaStream_t st) {
     static const bool want = getenv("VLY_MEGA_DBG") != nullptr;
     p.dbg = want ? kv->dbg : nullptr;
     g_mega_dbg = kv->dbg;
-  }
-  if (kv->umma) {
-    // tcgen05 consumer: swizzled activation block + ring of whole-box stages + barriers / handoff slots
-    p.Kmax = kv->umma_x_cols;
-    const size_t x_bytes = (size_t)(kv->umma_x_cols / 64) * 1024, stage_b = (size_t)kv->stage_bytes;
-    const size_t misc = ((1 + UmmaCfg::ISSUERS) * UmmaCfg::MAX_STAGES + 2 * UmmaCfg::ACC_SLOTS + 2 * UmmaCfg::RED_SLOTS + 2) * 8 + 16 +
-                        (size_t)UmmaCfg::RED_SLOTS * 4 * UmmaCfg::ROWS * bmax * 4 + (3 + 16) * bmax * 4 + 256;
-    int n_stages = (int)(((long long)227 * 1024 - 1024 - (long long)x_bytes - (long long)misc) / (long long)stage_b);
-    if (n_stages > UmmaCfg::MAX_STAGES) n_stages = UmmaCfg::MAX_STAGES;
-    static const int want = getenv("VLY_MEGA_STAGES") ? atoi(getenv("VLY_MEGA_STAGES")) : 0;
-    if (want > 0 && n_stages > want) n_stages = want;
-    if (n_stages < 2) return fail(VLY_ERR_INVALID, "decode (tcgen05 consumer): no room for the weight ring");
-    static const int inflight = getenv("VLY_MEGA_INFLIGHT") ? atoi(getenv("VLY_MEGA_INFLIGHT")) : 0;
-    p.n_stages = n_stages;
-    p.stage_bytes = (int)stage_b;
-    p.n_inflight = (inflight > 0 && inflight < n_stages) ? inflight : n_stages;
-    const size_t smem = x_bytes + (size_t)n_stages * stage_b + misc;
-    void* args[] = {&p};
-    cudaError_t e;
-    if (bmax == 2) {
-      TRY(ensure_smem_attr(c->cfg.device, decode_step_umma_kernel<2>, smem));
-      e = cudaLaunchCooperativeKernel((void*)decode_step_umma_kernel<2>, dim3(c->num_sms), dim3(MegaCfg::THREADS), args, smem, st);
-    } else {
-      TRY(ensure_smem_attr(c->cfg.device, decode_step_umma_kernel<4>, smem));
-      e = cudaLaunchCooperativeKernel((void*)decode_step_umma_kernel<4>, dim3(c->num_sms), dim3(MegaCfg::THREADS), args, smem, st);
-    }
-    c->launches++;
-    CK(e);
-    return VLY_OK;
   }
   size_t x_bytes, misc;
   mega_smem_layout(g, bmax, &x_bytes, &misc);

@@ -1,300 +1,32 @@
-// tcgen05 attention kernels.
+// wgmma attention kernels (sm_90a).
 //
-//  vit_attention_kernel    : CLIP ViT-L/14 self-attention (HF:modeling_clip.py:261-279, :300-336):
-//                            257 tokens, 16 heads x 64, no mask.  All 257 keys of a (frame, head) fit on
-//                            chip, so S = Q K^T for a 128-row query tile lives entirely in TMEM (272 fp32
-//                            columns), softmax is a single pass, P goes to shared memory as bf16 and
-//                            O = P V accumulates in TMEM.  V is consumed as an MN-major B operand straight
-//                            from the row-major QKV buffer (no transpose pass).
-//  llama_prefill_attention : causal attention with KV cache (HF:modeling_llama.py:199-222, :251-289),
-//                            head_dim 128, two-pass flash style: pass 1 computes the row max / sum over all
-//                            key blocks, pass 2 recomputes S, writes P = exp(s - max) and accumulates
-//                            O += P V in TMEM without rescaling.  Prefill attention is ~1% of prefill FLOPs
-//                            at S~340, so the recompute is irrelevant; what matters is exactness.
+//  vit_attention_kernel           : CLIP ViT-L/14 self-attention (HF:modeling_clip.py:261-279, :300-336): 257 tokens,
+//                                   16 heads x 64, no mask.  Q, K and V are read by TMA straight from the row-major QKV
+//                                   buffer (no transpose pass).
+//  llama_prefill_attention_kernel : causal attention with KV cache (HF:modeling_llama.py:199-222, :251-289), head_dim 128,
+//                                   HF's 2-D attention_mask as one bit per cache position.
+//
+// Both are the same flash-attention loop, one warpgroup per 64-row query tile:
+//   S = Q K^T        wgmma m64n64k16, Q and K K-major in shared memory (128-byte swizzle, TMA boxes of 64 rows x 64 columns)
+//   online softmax   in registers: each query row is held by the 4 lanes of a quad, row max / sum by two shuffles
+//   O += P V         wgmma m64n{HD}k16 with P as the REGISTER A operand (the S fragment layout is the A fragment layout) and
+//                    V as a transposed (MN-major) shared-memory B operand -- V is used exactly as it is stored.
+// K/V blocks of 64 keys are double-buffered: thread 0 issues the TMA loads of block j + 2 as soon as block j is consumed.
 #pragma once
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace vly {
 
-// Write 8 bf16 (16 B) of row `r`, columns [col, col+8) into a K-major SWIZZLE_128B operand made of
-// 64-column blocks of `rows_per_block` rows (block stride = rows_per_block * 128 B).
-VLY_DEVINL void st_sw128_row16(uint8_t* base, int rows_per_block, int r, int col, uint4 v) {
-  const int cb = col >> 6, c16 = (col & 63) >> 3;
-  uint8_t* p = base + (size_t)cb * rows_per_block * 128 + r * 128 + ((c16 ^ (r & 7)) << 4);
-  *reinterpret_cast<uint4*>(p) = v;
-}
-
-// ============================================================================================
-// ViT attention
-// ============================================================================================
 struct VitAttnParams {
   int F;                    // frames
   int tokens;               // 257
   int heads;                // 16
   int D;                    // 1024
   __nv_bfloat16* ctx;       // [F*tokens, D]
-  const __nv_bfloat16* qkv; // [F*tokens, 3D] (the tensor the TMA maps describe; the ping-pong kernel reads three single rows directly)
   float scale_log2e;        // head_dim^-0.5 * log2(e)
-  long long* dbg;           // optional cycle counters (profiling aid)
 };
 
-struct VitAttnCfg {
-  static constexpr int KEYS_PAD = 272;                    // 257 padded to a multiple of 16 (UMMA K step) and 8 (atom)
-  static constexpr int Q_BYTES = 128 * 128;               // 128 rows x 64 bf16
-  static constexpr int KV_BYTES = KEYS_PAD * 128;         // 272 rows x 64 bf16
-  static constexpr int P_BLOCKS = 5;                      // 272 key columns -> 5 blocks of 64
-  static constexpr int P_BYTES = P_BLOCKS * 128 * 128;
-  static constexpr int OFF_Q = 0;                         // two Q buffers
-  static constexpr int OFF_K = 2 * Q_BYTES;
-  static constexpr int OFF_V = OFF_K + KV_BYTES;
-  static constexpr int OFF_P = OFF_V + KV_BYTES;
-  static constexpr int OFF_BAR = OFF_P + P_BYTES;
-  static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
-  static constexpr int THREADS = 160;                     // warp 0: TMA + MMA issue; warps 1-4: softmax / epilogue
-  static constexpr int TMEM_COLS = 512;
-  static constexpr int O_COL = 320;
-};
-
-// tma_q : 2D map over qkv [F*257, 3*D], box {64, 128};  tma_kv : same tensor, box {64, 136}
-__global__ void __launch_bounds__(160, 1)
-vit_attention_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant__ CUtensorMap tma_kv,
-                     const VitAttnParams p) {
-  using C = VitAttnCfg;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base_u32 = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem = smem_raw + (base_u32 - smem_u32(smem_raw));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
-  uint64_t* kv_full = bars + 0;
-  uint64_t* q_full = bars + 1;   // [2]
-  uint64_t* s_full = bars + 3;
-  uint64_t* p_full = bars + 4;
-  uint64_t* o_full = bars + 5;
-  uint64_t* o_empty = bars + 6;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_items = p.F * p.heads;
-  const int n_qt = (p.tokens + 127) / 128;   // 3
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tma_q);
-    tma_prefetch_desc(&tma_kv);
-    mbar_init(kv_full, 1);
-    mbar_init(&q_full[0], 1);
-    mbar_init(&q_full[1], 1);
-    mbar_init(s_full, 1);
-    mbar_init(p_full, 128);
-    mbar_init(o_full, 1);
-    mbar_init(o_empty, 128);
-    fence_barrier_init();
-  }
-  if (warp == 0) {
-    __syncwarp();
-    tmem_alloc(tmem_slot, C::TMEM_COLS);
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s256 = make_idesc_bf16(128, 256);
-      constexpr uint32_t idesc_s16 = make_idesc_bf16(128, 16);
-      constexpr uint32_t idesc_pv = make_idesc_bf16(128, 64, 0, /*b MN-major*/ 1);
-      uint32_t kv_ph = 0, q_ph[2] = {0, 0}, p_ph = 0, oe_ph = 0;
-      uint32_t o_ph = (n_qt - 1) & 1;  // parity of the LAST o_full phase of the first item
-      int t_global = 0;  // running tile counter (selects the Q buffer)
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        const int f = item / p.heads, h = item % p.heads;
-        const int row0 = f * p.tokens;
-        // K and V of this (frame, head): rows row0 .. row0+271 (rows past the frame are masked / multiplied by 0)
-        mbar_expect_tx(kv_full, 2 * C::KV_BYTES);
-        tma_load_2d(smem + C::OFF_K, &tma_kv, kv_full, p.D + h * 64, row0);
-        tma_load_2d(smem + C::OFF_K + 136 * 128, &tma_kv, kv_full, p.D + h * 64, row0 + 136);
-        tma_load_2d(smem + C::OFF_V, &tma_kv, kv_full, 2 * p.D + h * 64, row0);
-        tma_load_2d(smem + C::OFF_V + 136 * 128, &tma_kv, kv_full, 2 * p.D + h * 64, row0 + 136);
-        // first Q tile
-        {
-          const int qb = t_global & 1;
-          mbar_expect_tx(&q_full[qb], C::Q_BYTES);
-          tma_load_2d(smem + C::OFF_Q + qb * C::Q_BYTES, &tma_q, &q_full[qb], h * 64, row0);
-        }
-        mbar_wait(kv_full, kv_ph);
-        kv_ph ^= 1;
-        for (int qt = 0; qt < n_qt; ++qt, ++t_global) {
-          const int qb = t_global & 1;
-          mbar_wait(&q_full[qb], q_ph[qb]);
-          q_ph[qb] ^= 1;
-          tc_fence_after();
-          // ---- S = Q K^T : K=64 -> 4 k-steps, N = 256 + 16 ----
-          const uint32_t q_addr = base_u32 + C::OFF_Q + qb * C::Q_BYTES;
-          const uint32_t k_addr = base_u32 + C::OFF_K;
-          const uint64_t dq = make_smem_desc_sw128(q_addr, 16, 1024);
-          const uint64_t dk0 = make_smem_desc_sw128(k_addr, 16, 1024);
-          const uint64_t dk1 = make_smem_desc_sw128(k_addr + 256 * 128, 16, 1024);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            tc_mma_bf16(tmem_base + 0, dq + 2 * k, dk0 + 2 * k, idesc_s256, k != 0);
-            tc_mma_bf16(tmem_base + 256, dq + 2 * k, dk1 + 2 * k, idesc_s16, k != 0);
-          }
-          tc_commit(s_full);
-          // prefetch the next Q tile of this item into the other buffer (its last reader, the S-MMA of
-          // tile t-1, completed before p_full(t-1) which we already waited on)
-          if (qt + 1 < n_qt) {
-            const int nb = (t_global + 1) & 1;
-            mbar_expect_tx(&q_full[nb], C::Q_BYTES);
-            tma_load_2d(smem + C::OFF_Q + nb * C::Q_BYTES, &tma_q, &q_full[nb], h * 64, row0 + (qt + 1) * 128);
-          }
-          // ---- wait for P (bf16 in smem), previous O drained ----
-          mbar_wait(p_full, p_ph);
-          p_ph ^= 1;
-          mbar_wait(o_empty, oe_ph ^ 1);
-          oe_ph ^= 1;
-          tc_fence_after();
-          // ---- O = P V : K = 272 keys -> 17 k-steps; A = P (K-major), B = V (MN-major, N = 64) ----
-          const uint32_t p_addr = base_u32 + C::OFF_P, v_addr = base_u32 + C::OFF_V;
-#pragma unroll 1
-          for (int j = 0; j < C::KEYS_PAD / 16; ++j) {
-            const uint64_t dp = make_smem_desc_sw128(p_addr + (j >> 2) * (128 * 128) + (j & 3) * 32, 16, 1024);
-            const uint64_t dv = make_smem_desc_sw128(v_addr + j * 16 * 128, 16, 1024);
-            tc_mma_bf16(tmem_base + C::O_COL, dp, dv, idesc_pv, j != 0);
-          }
-          tc_commit(o_full);
-        }
-        // K/V smem is overwritten by the next item: all PV MMAs must have retired
-        mbar_wait(o_full, o_ph);
-        o_ph ^= (n_qt & 1);   // o_full completes n_qt phases per item; we only observe the last one
-      }
-    }
-  } else {
-    // ================= softmax + epilogue: one query row per thread =================
-    const int quad = warp & 3;
-    const int r = quad * 32 + lane;
-    const uint32_t lane_addr = uint32_t(quad * 32) << 16;
-    uint32_t s_ph = 0, o_ph = 0;
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-      const int f = item / p.heads, h = item % p.heads;
-      for (int qt = 0; qt < n_qt; ++qt) {
-        const int qrow = qt * 128 + r;
-        const bool warp_active = (qt * 128 + quad * 32) < p.tokens;  // warp-uniform
-        __syncwarp();
-        mbar_wait(s_full, s_ph);
-        s_ph ^= 1;
-        tc_fence_after();
-        float row_sum = 1.f;
-        if (warp_active) {
-          // pass 1: row max over the 257 valid keys
-          float mx = -INFINITY;
-#pragma unroll 1
-          for (int c = 0; c < 8; ++c) {
-            uint32_t v[32];
-            tmem_ld_32x32(tmem_base + lane_addr + c * 32, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) mx = fmaxf(mx, __uint_as_float(v[i]));
-          }
-          {
-            uint32_t v[16];
-            tmem_ld_32x16(tmem_base + lane_addr + 256, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 16; ++i)
-              if (256 + i < p.tokens) mx = fmaxf(mx, __uint_as_float(v[i]));
-          }
-          const float mb = mx * p.scale_log2e;
-          // pass 2: p = exp2(s*scale*log2e - max*scale*log2e), write bf16 P, accumulate the row sum
-          float sum = 0.f;
-          uint8_t* sP = smem + C::OFF_P;
-#pragma unroll 1
-          for (int c = 0; c < 8; ++c) {
-            uint32_t v[32];
-            tmem_ld_32x32(tmem_base + lane_addr + c * 32, v);
-            tmem_ld_wait();
-            float e[32];
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              e[i] = fast_exp2(fmaf(__uint_as_float(v[i]), p.scale_log2e, -mb));
-              sum += e[i];
-            }
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              st_sw128_row16(sP, 128, r, c * 32 + j * 8,
-                             make_uint4(pack_bf16x2(e[8 * j], e[8 * j + 1]), pack_bf16x2(e[8 * j + 2], e[8 * j + 3]),
-                                        pack_bf16x2(e[8 * j + 4], e[8 * j + 5]), pack_bf16x2(e[8 * j + 6], e[8 * j + 7])));
-          }
-          {
-            uint32_t v[16];
-            tmem_ld_32x16(tmem_base + lane_addr + 256, v);
-            tmem_ld_wait();
-            float e[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              e[i] = (256 + i < p.tokens) ? fast_exp2(fmaf(__uint_as_float(v[i]), p.scale_log2e, -mb)) : 0.f;
-              sum += e[i];
-            }
-#pragma unroll
-            for (int j = 0; j < 2; ++j)
-              st_sw128_row16(sP, 128, r, 256 + j * 8,
-                             make_uint4(pack_bf16x2(e[8 * j], e[8 * j + 1]), pack_bf16x2(e[8 * j + 2], e[8 * j + 3]),
-                                        pack_bf16x2(e[8 * j + 4], e[8 * j + 5]), pack_bf16x2(e[8 * j + 6], e[8 * j + 7])));
-          }
-          row_sum = sum;
-        } else {
-          // rows past the last token: P must still be finite (0) so the MMA does not produce NaN garbage
-          uint8_t* sP = smem + C::OFF_P;
-          for (int col = 0; col < C::KEYS_PAD; col += 8) st_sw128_row16(sP, 128, r, col, make_uint4(0, 0, 0, 0));
-        }
-        // generic-proxy smem writes -> visible to the tensor core (async proxy); S fully consumed
-        fence_proxy_async_smem();
-        tc_fence_before();
-        mbar_arrive(p_full);
-
-        // ---- epilogue: O / sum -> ctx ----
-        __syncwarp();
-        mbar_wait(o_full, o_ph);
-        o_ph ^= 1;
-        tc_fence_after();
-        if (warp_active) {
-          const float inv = __frcp_rn(row_sum);
-          __nv_bfloat16* dst = p.ctx + ((size_t)f * p.tokens + qrow) * p.D + h * 64;
-#pragma unroll 1
-          for (int c = 0; c < 2; ++c) {
-            uint32_t v[32];
-            tmem_ld_32x32(tmem_base + lane_addr + C::O_COL + c * 32, v);
-            tmem_ld_wait();
-            if (qrow < p.tokens) {
-              uint4* op = reinterpret_cast<uint4*>(dst + c * 32);
-#pragma unroll
-              for (int j = 0; j < 4; ++j)
-                op[j] = make_uint4(
-                    pack_bf16x2(__uint_as_float(v[8 * j]) * inv, __uint_as_float(v[8 * j + 1]) * inv),
-                    pack_bf16x2(__uint_as_float(v[8 * j + 2]) * inv, __uint_as_float(v[8 * j + 3]) * inv),
-                    pack_bf16x2(__uint_as_float(v[8 * j + 4]) * inv, __uint_as_float(v[8 * j + 5]) * inv),
-                    pack_bf16x2(__uint_as_float(v[8 * j + 6]) * inv, __uint_as_float(v[8 * j + 7]) * inv));
-            }
-          }
-        }
-        __syncwarp();
-        tc_fence_before();
-        mbar_arrive(o_empty);
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, C::TMEM_COLS);
-  }
-}
-
-// ============================================================================================
-// LLaMA prefill attention (causal, head_dim 128, KV cache [B, nH, Smax, 128], q/k in the
-// RoPE-interleaved column order written by the QKV epilogue; v and the output in natural order)
-// ============================================================================================
 struct PrefillAttnParams {
   int B, S, past, nH, H, Smax;
   __nv_bfloat16* ctx;   // [B*S, H]
@@ -305,674 +37,231 @@ struct PrefillAttnParams {
   int mask_words;
 };
 
-struct PrefillAttnCfg {
-  static constexpr int TILE_BYTES = 128 * 128;             // 128 rows x 64 bf16 (one 64-col block)
-  static constexpr int OFF_Q = 0;                          // 2 blocks
-  static constexpr int OFF_K = 2 * TILE_BYTES;             // 2 stages x 2 blocks
-  static constexpr int OFF_V = OFF_K + 4 * TILE_BYTES;     // 2 stages x 2 blocks
-  static constexpr int OFF_P = OFF_V + 4 * TILE_BYTES;     // 2 blocks
-  static constexpr int OFF_BAR = OFF_P + 2 * TILE_BYTES;
-  static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
-  static constexpr int THREADS = 192;                      // warp 0 TMA, warp 1 MMA, warps 2-5 softmax
-  static constexpr int TMEM_COLS = 256;                    // S [0,128), O [128,256)
+template <int HD>
+struct FlashCfg {
+  static constexpr int BOX = 64 * 128;                     // 64 rows x 64 bf16 (one TMA box, 128-byte swizzle)
+  static constexpr int TILE = HD / 64 * BOX;               // 64 rows x HD
+  static constexpr int OFF_Q = 0;
+  static constexpr int OFF_K = TILE;                       // [2 stages]
+  static constexpr int OFF_V = OFF_K + 2 * TILE;           // [2 stages]
+  static constexpr int OFF_BAR = OFF_V + 2 * TILE;
+  static constexpr int SMEM_BYTES = OFF_BAR + 64 + 1024;   // + alignment slack
+  static constexpr int THREADS = 128;
 };
 
-// tma_q : 2D over qbuf [B*S, H], box {64,128};  tma_k / tma_v : 3D over cache {128, Smax, B*nH}, box {64,128,1}
-__global__ void __launch_bounds__(192, 1)
+// The shared loop.  load_kv(j, stage) issues the TMA loads of key block j (K and V, 2 * TILE bytes) on kv_full[stage];
+// key_ok(row, key) says whether query row `row` (0..63 of the tile) may attend key `key`; finish(row, col, o0, o1) stores two
+// adjacent output columns of a row (already divided by the row sum).
+template <int HD, typename LoadKV, typename KeyOk, typename Finish>
+VLY_DEVINL void flash_attention_tile(uint8_t* smem, uint32_t base_u32, uint64_t* q_full, uint64_t* kv_full, int nkv, float scale_log2e,
+                                     LoadKV load_kv, KeyOk key_ok, Finish finish) {
+  using C = FlashCfg<HD>;
+  constexpr int OR = HD / 2;                               // O accumulator registers per thread
+  const int t = threadIdx.x, w = t >> 5, l = t & 31;
+  const int r_lo = w * 16 + (l >> 2), c_lo = (l & 3) * 2;  // fragment row (and r_lo + 8), first column of each 8-column group
+  float o[OR];
+#pragma unroll
+  for (int i = 0; i < OR; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, lsum[2] = {0.f, 0.f};
+  const uint64_t desc_q = make_smem_desc_sw128(base_u32 + C::OFF_Q, 16, 1024);
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < nkv; ++j) {
+    const int st = j & 1;
+    mbar_wait(&kv_full[st], (j >> 1) & 1);
+    // ---- S = Q K^T ----
+    float s[32];
+    const uint64_t desc_k = make_smem_desc_sw128(base_u32 + C::OFF_K + st * C::TILE, 16, 1024);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < HD / 16; ++kk) {
+      const uint64_t off = uint64_t((kk >> 2) * (C::BOX / 16) + (kk & 3) * 2);
+      wgmma_ss_n64(s, desc_q + off, desc_k + off, kk != 0);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    // ---- mask + online softmax (scores in log2 units) ----
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int g = 0; g < 8; ++g)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int row = r_lo + 8 * (i >> 1), key = j * 64 + g * 8 + c_lo + (i & 1);
+        const float v = key_ok(row, key) ? s[4 * g + i] * scale_log2e : -INFINITY;
+        s[4 * g + i] = v;
+        mx[i >> 1] = fmaxf(mx[i >> 1], v);
+      }
+    float alpha[2], mb[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+      const float mn = fmaxf(m[h], mx[h]);
+      mb[h] = mn > -INFINITY ? mn : 0.f;                   // a row with nothing visible yet keeps p = 0 and no NaN
+      alpha[h] = fast_exp2(m[h] - mb[h]);                  // m = -inf -> 0 (o and lsum are 0 then anyway)
+      m[h] = mn;
+      lsum[h] *= alpha[h];
+    }
+#pragma unroll
+    for (int g = 0; g < OR / 4; ++g) {
+      o[4 * g] *= alpha[0]; o[4 * g + 1] *= alpha[0];
+      o[4 * g + 2] *= alpha[1]; o[4 * g + 3] *= alpha[1];
+    }
+    uint32_t pa[4][4];                                     // P as bf16 A fragments, one per 16 keys
+#pragma unroll
+    for (int g = 0; g < 8; ++g) {
+      const float p0 = fast_exp2(s[4 * g] - mb[0]), p1 = fast_exp2(s[4 * g + 1] - mb[0]);
+      const float p2 = fast_exp2(s[4 * g + 2] - mb[1]), p3 = fast_exp2(s[4 * g + 3] - mb[1]);
+      lsum[0] += p0 + p1;
+      lsum[1] += p2 + p3;
+      pa[g >> 1][(g & 1) * 2] = pack_bf16x2(p0, p1);
+      pa[g >> 1][(g & 1) * 2 + 1] = pack_bf16x2(p2, p3);
+    }
+    // ---- O += P V ----
+    const uint64_t desc_v = make_smem_desc_sw128(base_u32 + C::OFF_V + st * C::TILE, C::BOX, 1024);
+    wgmma_fence_regs(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {                       // 16 keys = two 1024-byte atoms of V
+      if constexpr (HD == 64) wgmma_rs_n64_tb(*reinterpret_cast<float(*)[32]>(o), pa[kk], desc_v + uint64_t(kk * 128), 1);
+      else wgmma_rs_n128_tb(*reinterpret_cast<float(*)[64]>(o), pa[kk], desc_v + uint64_t(kk * 128), 1);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    __syncthreads();                                       // every warp is done with this stage
+    if (t == 0 && j + 2 < nkv) load_kv(j + 2, st);
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    lsum[h] += __shfl_xor_sync(0xffffffffu, lsum[h], 1);
+    lsum[h] += __shfl_xor_sync(0xffffffffu, lsum[h], 2);
+  }
+  const float inv0 = lsum[0] > 0.f ? __frcp_rn(lsum[0]) : 0.f;   // fully masked query row -> zeros (its output is never attended)
+  const float inv1 = lsum[1] > 0.f ? __frcp_rn(lsum[1]) : 0.f;
+#pragma unroll
+  for (int g = 0; g < OR / 4; ++g) {
+    finish(r_lo, g * 8 + c_lo, o[4 * g] * inv0, o[4 * g + 1] * inv0);
+    finish(r_lo + 8, g * 8 + c_lo, o[4 * g + 2] * inv1, o[4 * g + 3] * inv1);
+  }
+}
+
+VLY_DEVINL uint8_t* flash_smem(uint32_t* base_u32) {
+  extern __shared__ uint8_t smem_raw[];
+  *base_u32 = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  return smem_raw + (*base_u32 - smem_u32(smem_raw));
+}
+
+// ============================================================================================
+// ViT attention.  grid = F * heads * ceil(tokens / 64); tma_qkv: 2D map over qkv [F*tokens, 3*D], box {64, 64}.
+// Rows of a box past the frame belong to the next frame (or are zero-filled past the tensor): their keys are masked, their
+// query rows are not stored.
+// ============================================================================================
+__global__ void __launch_bounds__(128, 1)
+vit_attention_kernel(const __grid_constant__ CUtensorMap tma_qkv, const VitAttnParams p) {
+  using C = FlashCfg<64>;
+  uint32_t base_u32;
+  uint8_t* smem = flash_smem(&base_u32);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
+  uint64_t* q_full = bars;
+  uint64_t* kv_full = bars + 1;   // [2]
+  const int n_qt = (p.tokens + 63) / 64;
+  const int qt = blockIdx.x % n_qt, item = blockIdx.x / n_qt;
+  const int f = item / p.heads, h = item % p.heads;
+  const int row0 = f * p.tokens;
+  const int nkv = n_qt;
+  auto load_kv = [&](int j, int st) {
+    mbar_expect_tx(&kv_full[st], 2 * C::TILE);
+    tma_load_2d(smem + C::OFF_K + st * C::TILE, &tma_qkv, &kv_full[st], p.D + h * 64, row0 + j * 64);
+    tma_load_2d(smem + C::OFF_V + st * C::TILE, &tma_qkv, &kv_full[st], 2 * p.D + h * 64, row0 + j * 64);
+  };
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tma_qkv);
+    mbar_init(q_full, 1);
+    mbar_init(&kv_full[0], 1);
+    mbar_init(&kv_full[1], 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  pdl_launch_dependents();
+  if (threadIdx.x == 0) {
+    pdl_wait();                   // the QKV GEMM's output is read by the TMA loads below
+    mbar_expect_tx(q_full, C::TILE);
+    tma_load_2d(smem + C::OFF_Q, &tma_qkv, q_full, h * 64, row0 + qt * 64);
+    load_kv(0, 0);
+    if (nkv > 1) load_kv(1, 1);
+  }
+  const int tokens = p.tokens;
+  flash_attention_tile<64>(
+      smem, base_u32, q_full, kv_full, nkv, p.scale_log2e, load_kv, [&](int, int key) { return key < tokens; },
+      [&](int r, int col, float o0, float o1) {
+        const int q = qt * 64 + r;
+        if (q < tokens)
+          *reinterpret_cast<uint32_t*>(p.ctx + ((size_t)f * tokens + q) * p.D + h * 64 + col) = pack_bf16x2(o0, o1);
+      });
+}
+
+// ============================================================================================
+// LLaMA prefill attention (causal, head_dim 128, KV cache [B, nH, Smax, 128], q/k in the RoPE-interleaved column order
+// written by the QKV epilogue -- the same permutation on both sides of the dot product; v and the output in natural order).
+// grid = B * nH * ceil(S / 64).  tma_q: 2D over qbuf [B*S, H], box {64, 64};  tma_k / tma_v: 3D over the cache
+// {128, Smax, B*nH}, box {64, 64, 1}.
+// ============================================================================================
+__global__ void __launch_bounds__(128, 1)
 llama_prefill_attention_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant__ CUtensorMap tma_k,
                                const __grid_constant__ CUtensorMap tma_v, const PrefillAttnParams p) {
-  using C = PrefillAttnCfg;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base_u32 = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* smem = smem_raw + (base_u32 - smem_u32(smem_raw));
+  using C = FlashCfg<128>;
+  uint32_t base_u32;
+  uint8_t* smem = flash_smem(&base_u32);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
-  uint64_t* q_full = bars + 0;
-  uint64_t* kv_full = bars + 1;    // [2]
-  uint64_t* kv_empty = bars + 3;   // [2]
-  uint64_t* s_full = bars + 5;
-  uint64_t* s_empty = bars + 6;
-  uint64_t* p_full = bars + 7;
-  uint64_t* p_empty = bars + 8;
-  uint64_t* o_full = bars + 9;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 10);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_qt = (p.S + 127) / 128;
+  uint64_t* q_full = bars;
+  uint64_t* kv_full = bars + 1;   // [2]
+  const int n_qt = (p.S + 63) / 64;
   const int qt = blockIdx.x % n_qt;
   const int bh = blockIdx.x / n_qt;          // b * nH + h
   const int b = bh / p.nH, h = bh % p.nH;
   const int kv_len = p.past + p.S;
-  const int q_hi = min(p.S, (qt + 1) * 128);                 // one past the last query row of this tile
-  const int nkv = (p.past + q_hi + 127) / 128;               // key blocks any row of the tile can see
-  const int n_iter = 2 * nkv;
-
+  const int q_hi = min(p.S, (qt + 1) * 64);                  // one past the last query row of this tile
+  const int nkv = (p.past + q_hi + 63) / 64;                 // key blocks any row of the tile can see
+  auto load_kv = [&](int j, int st) {
+    mbar_expect_tx(&kv_full[st], 2 * C::TILE);
+    uint8_t* kd = smem + C::OFF_K + st * C::TILE;
+    uint8_t* vd = smem + C::OFF_V + st * C::TILE;
+    tma_load_3d(kd, &tma_k, &kv_full[st], 0, j * 64, bh);
+    tma_load_3d(kd + C::BOX, &tma_k, &kv_full[st], 64, j * 64, bh);
+    tma_load_3d(vd, &tma_v, &kv_full[st], 0, j * 64, bh);
+    tma_load_3d(vd + C::BOX, &tma_v, &kv_full[st], 64, j * 64, bh);
+  };
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tma_q);
     tma_prefetch_desc(&tma_k);
     tma_prefetch_desc(&tma_v);
     mbar_init(q_full, 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&kv_full[i], 1);
-      mbar_init(&kv_empty[i], 1);
-    }
-    mbar_init(s_full, 1);
-    mbar_init(s_empty, 128);
-    mbar_init(p_full, 128);
-    mbar_init(p_empty, 1);
-    mbar_init(o_full, 1);
+    mbar_init(&kv_full[0], 1);
+    mbar_init(&kv_full[1], 1);
     fence_barrier_init();
   }
-  if (warp == 1) {
-    __syncwarp();
-    tmem_alloc(tmem_slot, C::TMEM_COLS);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
   pdl_launch_dependents();
-  if (warp == 0) {
-    if (lane == 0) {
-      pdl_wait();               // q and the appended K/V rows come from the QKV GEMM of this layer
-      mbar_expect_tx(q_full, 2 * C::TILE_BYTES);
-      tma_load_2d(smem + C::OFF_Q, &tma_q, q_full, h * 128, b * p.S + qt * 128);
-      tma_load_2d(smem + C::OFF_Q + C::TILE_BYTES, &tma_q, q_full, h * 128 + 64, b * p.S + qt * 128);
-      int st = 0;
-      uint32_t ph = 0;
-      for (int it = 0; it < n_iter; ++it) {
-        const int j = it % nkv, pass = it / nkv;
-        mbar_wait(&kv_empty[st], ph ^ 1);
-        mbar_expect_tx(&kv_full[st], (pass ? 4 : 2) * C::TILE_BYTES);
-        uint8_t* kd = smem + C::OFF_K + st * 2 * C::TILE_BYTES;
-        tma_load_3d(kd, &tma_k, &kv_full[st], 0, j * 128, bh);
-        tma_load_3d(kd + C::TILE_BYTES, &tma_k, &kv_full[st], 64, j * 128, bh);
-        if (pass) {
-          uint8_t* vd = smem + C::OFF_V + st * 2 * C::TILE_BYTES;
-          tma_load_3d(vd, &tma_v, &kv_full[st], 0, j * 128, bh);
-          tma_load_3d(vd + C::TILE_BYTES, &tma_v, &kv_full[st], 64, j * 128, bh);
-        }
-        if (++st == 2) { st = 0; ph ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, 128);
-      constexpr uint32_t idesc_pv = make_idesc_bf16(128, 128, 0, 1);
-      // descriptors are built once; the issue loop only advances their 16-byte-unit address field
-      const uint64_t desc_q = make_smem_desc_sw128(base_u32 + C::OFF_Q, 16, 1024);
-      const uint64_t desc_p = make_smem_desc_sw128(base_u32 + C::OFF_P, 16, 1024);
-      const uint64_t desc_k[2] = {make_smem_desc_sw128(base_u32 + C::OFF_K, 16, 1024),
-                                  make_smem_desc_sw128(base_u32 + C::OFF_K + 2 * C::TILE_BYTES, 16, 1024)};
-      const uint64_t desc_v[2] = {make_smem_desc_sw128(base_u32 + C::OFF_V, C::TILE_BYTES, 1024),
-                                  make_smem_desc_sw128(base_u32 + C::OFF_V + 2 * C::TILE_BYTES, C::TILE_BYTES, 1024)};
-      mbar_wait(q_full, 0);
-      int st = 0;
-      uint32_t ph = 0, se_ph = 0, pf_ph = 0;
-      for (int it = 0; it < n_iter; ++it) {
-        const int j = it % nkv, pass = it / nkv;
-        mbar_wait(&kv_full[st], ph);
-        mbar_wait(s_empty, se_ph ^ 1);   // softmax finished reading the previous S
-        se_ph ^= 1;
-        tc_fence_after();
-        {
-          const uint64_t dk = desc_k[st];
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk) {
-            const uint64_t off = uint64_t((kk >> 2) * (C::TILE_BYTES / 16) + (kk & 3) * 2);
-            tc_mma_bf16(tmem_base + 0, desc_q + off, dk + off, idesc_s, kk != 0);
-          }
-        }
-        tc_commit(s_full);
-        if (!pass) {
-          tc_commit(&kv_empty[st]);
-        } else {
-          mbar_wait(p_full, pf_ph);
-          pf_ph ^= 1;
-          tc_fence_after();
-          const uint64_t dv = desc_v[st];
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk) {
-            // A = P[128 rows, keys kk*16..+16): key block (kk>>2), 32 B per k-step inside the atom
-            // B = V[keys kk*16..+16, d 0..127] MN-major: 16 keys = 2 atoms of 1024 B; d chunks 16 KB apart (LBO)
-            tc_mma_bf16(tmem_base + 128, desc_p + uint64_t((kk >> 2) * (C::TILE_BYTES / 16) + (kk & 3) * 2),
-                        dv + uint64_t(kk * (16 * 128 / 16)), idesc_pv, (j | kk) != 0);
-          }
-          tc_commit(&kv_empty[st]);
-          tc_commit(p_empty);
-          if (it == n_iter - 1) tc_commit(o_full);
-        }
-        if (++st == 2) { st = 0; ph ^= 1; }
-      }
-    }
-  } else {
-    const int quad = warp & 3;
-    const int r = quad * 32 + lane;
-    const uint32_t lane_addr = uint32_t(quad * 32) << 16;
-    const int q_idx = qt * 128 + r;           // query index within the sequence
-    const int q_pos = p.past + q_idx;         // absolute position
-    uint32_t sf_ph = 0, pe_ph = 0;
-    float m = -INFINITY, l = 0.f;
-    const uint32_t* kbits = p.key_bits ? p.key_bits + (size_t)b * p.mask_words : nullptr;
-    // ---------------- pass 1: running max / sum ----------------
-    for (int j = 0; j < nkv; ++j) {
-      __syncwarp();
-      mbar_wait(s_full, sf_ph);
-      sf_ph ^= 1;
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + lane_addr + c * 32, v);
-        tmem_ld_wait();
-        const uint32_t kb = kbits ? __ldg(kbits + j * 4 + c) : 0xffffffffu;
-        float s[32], cm = -INFINITY;
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const int key = j * 128 + c * 32 + i;
-          s[i] = (key <= q_pos && key < kv_len && ((kb >> i) & 1u)) ? __uint_as_float(v[i]) * p.scale_log2e : -INFINITY;
-          cm = fmaxf(cm, s[i]);
-        }
-        const float mn = fmaxf(m, cm);
-        if (mn > -INFINITY) {
-          float acc = 0.f;
-#pragma unroll
-          for (int i = 0; i < 32; ++i) acc += fast_exp2(s[i] - mn);
-          l = l * fast_exp2(m - mn) + acc;
-          m = mn;
-        }
-      }
-      __syncwarp();
-      tc_fence_before();
-      mbar_arrive(s_empty);
-    }
-    // ---------------- pass 2: P = exp2(s - m) -> smem, O += P V ----------------
-    uint8_t* sP = smem + C::OFF_P;
-    for (int j = 0; j < nkv; ++j) {
-      __syncwarp();
-      mbar_wait(s_full, sf_ph);
-      sf_ph ^= 1;
-      mbar_wait(p_empty, pe_ph ^ 1);   // previous PV MMAs no longer read sP
-      pe_ph ^= 1;
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + lane_addr + c * 32, v);
-        tmem_ld_wait();
-        // a row whose every visible key is masked (a left-padding query) keeps m = -inf: kb is forced to 0 there, so e = 0
-        const uint32_t kb = m > -INFINITY ? (kbits ? __ldg(kbits + j * 4 + c) : 0xffffffffu) : 0u;
-        float e[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const int key = j * 128 + c * 32 + i;
-          e[i] = (key <= q_pos && key < kv_len && ((kb >> i) & 1u)) ? fast_exp2(fmaf(__uint_as_float(v[i]), p.scale_log2e, -m)) : 0.f;
-        }
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj)
-          st_sw128_row16(sP, 128, r, c * 32 + jj * 8,
-                         make_uint4(pack_bf16x2(e[8 * jj], e[8 * jj + 1]), pack_bf16x2(e[8 * jj + 2], e[8 * jj + 3]),
-                                    pack_bf16x2(e[8 * jj + 4], e[8 * jj + 5]), pack_bf16x2(e[8 * jj + 6], e[8 * jj + 7])));
-      }
-      __syncwarp();
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(s_empty);
-      mbar_arrive(p_full);
-    }
-    // ---------------- epilogue ----------------
-    __syncwarp();
-    mbar_wait(o_full, 0);
-    tc_fence_after();
-    const float inv = l > 0.f ? __frcp_rn(l) : 0.f;     // fully masked query row -> zeros (its output is never attended)
-    __nv_bfloat16* dst = p.ctx + ((size_t)b * p.S + q_idx) * p.H + h * 128;
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-      uint32_t v[32];
-      tmem_ld_32x32(tmem_base + lane_addr + 128 + c * 32, v);
-      tmem_ld_wait();
-      if (q_idx < p.S) {
-        uint4* op = reinterpret_cast<uint4*>(dst + c * 32);
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj)
-          op[jj] = make_uint4(
-              pack_bf16x2(__uint_as_float(v[8 * jj]) * inv, __uint_as_float(v[8 * jj + 1]) * inv),
-              pack_bf16x2(__uint_as_float(v[8 * jj + 2]) * inv, __uint_as_float(v[8 * jj + 3]) * inv),
-              pack_bf16x2(__uint_as_float(v[8 * jj + 4]) * inv, __uint_as_float(v[8 * jj + 5]) * inv),
-              pack_bf16x2(__uint_as_float(v[8 * jj + 6]) * inv, __uint_as_float(v[8 * jj + 7]) * inv));
-      }
-    }
-    __syncwarp();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, C::TMEM_COLS);
-  }
-}
-
-
-// ============================================================================================
-// ViT attention, generation 2: ping-pong pipeline.
-//   warp 0 (one thread)  : TMA loads + every tcgen05.mma
-//   warps 1-8 / 9-16     : softmax + epilogue warpgroups A / B, two threads per query row (each half of the keys)
-//   TMEM region R (256 columns each): S_R = Q K^T over keys 0..255 (UMMA 128x256x16 x4); O_R (64 columns) aliases the
-//   last 64 columns of S_R once P_R is complete.  Tiles alternate between the regions, so the softmax of one tile
-//   (MUFU-bound) overlaps the MMAs, TMEM traffic and epilogue of the other.  The 257th key (the CLS/last token)
-//   is handled on CUDA cores -- one 64-wide dot product and one axpy per row -- which keeps the MMA shapes clean
-//   (N = 256, K = 256) and removes the 272-column padding.  K is reloaded for the next (frame, head) as soon as the
-//   item's last S-MMA retires, V when its last P V retires.
-//   warp 17              : the 257th QUERY row of every (frame, head) on CUDA cores, straight from the K / V tiles in shared
-//   memory (64 conflict-free 16-byte loads for the scores, 128 8-byte loads for P V per lane): a third 128-row query tile with
-//   ONE valid row cost a full trip through the S-MMA / softmax / P V / epilogue chain, and the chain's latency -- not MUFU or
-//   issue slots -- is what bounds this kernel.  Two tiles per item also pin query tile 0 to warpgroup A and tile 1 to B.
-// ============================================================================================
-struct VitAttnPPCfg {
-  static constexpr int Q_BYTES = 128 * 128;
-  static constexpr int KV_BYTES = 256 * 128;
-  static constexpr int P_BYTES = 4 * 128 * 128;            // 256 key columns = 4 blocks of 64
-  static constexpr int OFF_Q = 0;                          // [2]
-  static constexpr int OFF_K = 2 * Q_BYTES;
-  static constexpr int OFF_V = OFF_K + KV_BYTES;
-  static constexpr int OFF_P = OFF_V + KV_BYTES;           // [2]
-  static constexpr int OFF_X = OFF_P + 2 * P_BYTES;        // 257th key / value rows per region: kx[128 B], vx[2 tile parities][128 B]
-  static constexpr int OFF_XMAX = OFF_X + 2 * 384;         // row max exchange between the two halves: [2 regions][2 halves][128] bf16
-  static constexpr int OFF_XSUM = OFF_XMAX + 1024;         // partial row sum of half 1: [2 regions][128] fp32
-  static constexpr int OFF_BAR = OFF_XSUM + 1024;
-  // 227 KB is the hard limit: there is no room for an alignment slack, the kernel traps if the dynamic shared memory
-  // window is not 1024-byte aligned (it is when the kernel has no static shared memory)
-  static constexpr int SMEM_BYTES = OFF_BAR + 128;
-  static constexpr int THREADS = 576;                      // warp 0 + two softmax warpgroups of 8 warps + the last-row warp
-  static constexpr int TPI = 2;                            // 128-row query tiles per (frame, head): rows 0..255; row 256 -> warp 17
-  static constexpr int TMEM_COLS = 512;
-  static constexpr int O_OFF = 192;
-};
-static_assert(VitAttnPPCfg::SMEM_BYTES <= 232448, "ViT attention exceeds 227 KB of shared memory");
-
-// tma_q: 2D over qkv [F*257, 3D], box {64,128};  tma_x: same tensor, box {64,1}
-__global__ void __launch_bounds__(576, 1)
-vit_attention_pp_kernel(const __grid_constant__ CUtensorMap tma_q, const __grid_constant__ CUtensorMap tma_x, const VitAttnParams p) {
-  using C = VitAttnPPCfg;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t base_u32 = smem_u32(smem_raw);
-  if (base_u32 & 1023u) __trap();          // SWIZZLE_128B operands need 1024-byte alignment; no slack left to fix it up
-  uint8_t* smem = smem_raw;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
-  uint64_t* k_full = bars + 0;
-  uint64_t* v_full = bars + 1;
-  uint64_t* k_done = bars + 2;
-  uint64_t* v_done = bars + 3;
-  uint64_t* q_full = bars + 4;    // [2]
-  uint64_t* s_full = bars + 6;    // [2]
-  uint64_t* p_full = bars + 8;    // [2]
-  uint64_t* o_full = bars + 10;   // [2]
-  uint64_t* r_free = bars + 12;   // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 14);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_items_total = p.F * p.heads;
-  const int my_items = (n_items_total > (int)blockIdx.x) ? (n_items_total - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
-  constexpr int TPI = C::TPI;
-  const int n_tiles = my_items * TPI;
-
   if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tma_q);
-    tma_prefetch_desc(&tma_x);
-    mbar_init(k_full, 1);
-    mbar_init(v_full, 1);
-    mbar_init(k_done, 2);       // the item's last S-MMA has retired (tcgen05.commit) AND warp 17 has read K
-    mbar_init(v_done, 2);       // the item's last P V has retired AND warp 17 has read V
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&q_full[i], 1);
-      mbar_init(&s_full[i], 1);
-      mbar_init(&p_full[i], 256);
-      mbar_init(&o_full[i], 1);
-      mbar_init(&r_free[i], 128);
-    }
-    fence_barrier_init();
+    pdl_wait();                   // q and the appended K/V rows come from the QKV GEMM of this layer
+    mbar_expect_tx(q_full, C::TILE);
+    tma_load_2d(smem + C::OFF_Q, &tma_q, q_full, h * 128, b * p.S + qt * 64);
+    tma_load_2d(smem + C::OFF_Q + C::BOX, &tma_q, q_full, h * 128 + 64, b * p.S + qt * 64);
+    load_kv(0, 0);
+    if (nkv > 1) load_kv(1, 1);
   }
-  if (warp == 0) {
-    __syncwarp();
-    tmem_alloc(tmem_slot, C::TMEM_COLS);
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  pdl_launch_dependents();      // (see gemm_tc_kernel: prologue overlaps the previous kernel's tail under programmatic launch)
-  if (warp == 0) {
-    if (lane == 0 && n_tiles > 0) {
-      pdl_wait();               // the QKV GEMM's output is read by the TMA loads below
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, 256);
-      constexpr uint32_t idesc_pv = make_idesc_bf16(128, 64, 0, 1);
-      const uint64_t desc_q[2] = {make_smem_desc_sw128(base_u32 + C::OFF_Q, 16, 1024), make_smem_desc_sw128(base_u32 + C::OFF_Q + C::Q_BYTES, 16, 1024)};
-      const uint64_t desc_p[2] = {make_smem_desc_sw128(base_u32 + C::OFF_P, 16, 1024), make_smem_desc_sw128(base_u32 + C::OFF_P + C::P_BYTES, 16, 1024)};
-      const uint64_t desc_k = make_smem_desc_sw128(base_u32 + C::OFF_K, 16, 1024);
-      const uint64_t desc_v = make_smem_desc_sw128(base_u32 + C::OFF_V, 16, 1024);
-      uint32_t kf_ph = 0, vf_ph = 0, kd_ph = 0, vd_ph = 0, q_ph[2] = {0, 0}, p_ph[2] = {0, 0}, rf_ph[2] = {0, 0};
-      long long w_vf = 0, w_pf = 0, w_vd = 0, w_rf = 0, w_kf = 0, w_qf = 0, w_kd = 0, x_mma = 0, x_tma = 0; const long long t_begin = clock64();
-      auto item_of = [&](int g) { return (int)blockIdx.x + (g / TPI) * (int)gridDim.x; };
-      auto load_k = [&](int item, int par) {
-        const int f = item / p.heads, h = item % p.heads, row0 = f * p.tokens;
-        mbar_expect_tx(k_full, C::KV_BYTES);
-        tma_load_2d(smem + C::OFF_K, &tma_q, k_full, p.D + h * 64, row0);
-        tma_load_2d(smem + C::OFF_K + 128 * 128, &tma_q, k_full, p.D + h * 64, row0 + 128);
-      };
-      auto load_v = [&](int item, int par) {
-        const int f = item / p.heads, h = item % p.heads, row0 = f * p.tokens;
-        mbar_expect_tx(v_full, C::KV_BYTES);
-        tma_load_2d(smem + C::OFF_V, &tma_q, v_full, 2 * p.D + h * 64, row0);
-        tma_load_2d(smem + C::OFF_V + 128 * 128, &tma_q, v_full, 2 * p.D + h * 64, row0 + 128);
-      };
-      auto back = [&](int t) {     // O = P V for tile t
-        const int R = t & 1;
-        if (t % TPI == 0) {        // first tile of an item: its V must have landed
-          { const long long tq_ = clock64(); mbar_wait(v_full, vf_ph); w_vf += clock64() - tq_; }
-          vf_ph ^= 1;
-        }
-        { const long long tq_ = clock64(); mbar_wait(&p_full[R], p_ph[R]); w_pf += clock64() - tq_; }
-        p_ph[R] ^= 1;
-        tc_fence_after();
-        // the single issuing thread must sustain one MMA per ~32 cycles here (N = 64): descriptors are precomputed and
-        // only their 16-byte-unit address field is advanced by compile-time constants
-        const uint64_t dp0 = desc_p[R];
-        const uint32_t d_o = tmem_base + R * 256 + C::O_OFF;
-        const long long tm_ = clock64();
-#pragma unroll
-        for (int j = 0; j < 16; ++j)
-          tc_mma_bf16(d_o, dp0 + uint64_t((j >> 2) * (128 * 128 / 16) + (j & 3) * 2), desc_v + uint64_t(j * (16 * 128 / 16)), idesc_pv, j != 0);
-        tc_commit(&o_full[R]);
-        x_mma += clock64() - tm_;
-        if (t % TPI == TPI - 1) tc_commit(v_done);      // every P V of the item has been issued
-      };
-      // Q tile + the 257th key / value rows of the (frame, head) travel together on the region's q_full barrier.  They are
-      // issued one tile AHEAD: Q_R / X_R[parity] are free as soon as p_full of the region's previous tile was observed.
-      auto issue_q = [&](int g) {
-        const int R = g & 1, qt = g % TPI, item = item_of(g);
-        const int f = item / p.heads, h = item % p.heads, row0 = f * p.tokens;
-        uint8_t* xr = smem + C::OFF_X + R * 384;       // kx: read before p_full; vx: read in the epilogue -> double buffered
-        mbar_expect_tx(&q_full[R], C::Q_BYTES + 256);
-        tma_load_2d(smem + C::OFF_Q + R * C::Q_BYTES, &tma_q, &q_full[R], h * 64, row0 + qt * 128);
-        tma_load_2d(xr, &tma_x, &q_full[R], p.D + h * 64, row0 + 256);
-        tma_load_2d(xr + 128 + ((g >> 1) & 1) * 128, &tma_x, &q_full[R], 2 * p.D + h * 64, row0 + 256);
-      };
-      load_k(item_of(0), 0);
-      load_v(item_of(0), 0);
-      issue_q(0);
-      for (int g = 0; g < n_tiles; ++g) {
-        const int R = g & 1, qt = g % TPI, item = item_of(g);
-        if (qt == 0 && g > 0) {
-          // the previous item's last P V is still pending: issue it, then its V buffer can be refilled
-          back(g - 1);
-          { const long long tq_ = clock64(); mbar_wait(v_done, vd_ph); w_vd += clock64() - tq_; }
-          vd_ph ^= 1;
-          load_v(item, (g / TPI) & 1);
-        }
-        { const long long tq_ = clock64(); mbar_wait(&r_free[R], rf_ph[R] ^ 1); w_rf += clock64() - tq_; }     // region R (S/O columns, Q_R, P_R) released by the epilogue of tile g-2
-        rf_ph[R] ^= 1;
-        if (qt == 0) {
-          { const long long tq_ = clock64(); mbar_wait(k_full, kf_ph); w_kf += clock64() - tq_; }
-          kf_ph ^= 1;
-        }
-        { const long long tq_ = clock64(); mbar_wait(&q_full[R], q_ph[R]); w_qf += clock64() - tq_; }
-        q_ph[R] ^= 1;
-        tc_fence_after();
-        {
-          const uint64_t dq = desc_q[R];
-          const long long tm_ = clock64();
-#pragma unroll
-          for (int k = 0; k < 4; ++k) tc_mma_bf16(tmem_base + R * 256, dq + 2 * k, desc_k + 2 * k, idesc_s, k != 0);
-          tc_commit(&s_full[R]);
-          x_mma += clock64() - tm_;
-        }
-        if (qt == TPI - 1) {
-          tc_commit(k_done);
-          if (g + 1 < n_tiles) {                 // refill K for the next item while this item's softmax / P V run
-            { const long long tq_ = clock64(); mbar_wait(k_done, kd_ph); w_kd += clock64() - tq_; }
-            kd_ph ^= 1;
-            load_k(item_of(g + 1), ((g + 1) / TPI) & 1);
-          }
-        }
-        if (qt != 0 && g > 0) back(g - 1);       // (for qt == 0 it was issued above)
-        if (g + 1 < n_tiles) { const long long tt_ = clock64(); issue_q(g + 1); x_tma += clock64() - tt_; }   // p_full(g-1) observed -> the other region's Q buffer is free
-      }
-      back(n_tiles - 1);
-      // all MMAs must retire before the CTA exits / TMEM is released
-      mbar_wait(v_done, vd_ph);
-      if (p.dbg) { long long* o = p.dbg + (size_t)blockIdx.x * 16; o[0] = clock64() - t_begin; o[1] = w_rf; o[2] = w_qf; o[3] = w_kf; o[4] = w_kd; o[5] = w_pf; o[6] = x_mma; o[7] = x_tma; }
-    }
-  } else if (warp <= 16) {
-    // ================= softmax + epilogue warpgroups: 8 warps each, TWO threads per query row =================
-    // thread (row r, half hf) owns key columns [128*hf, 128*hf+128) of S; half 0 also owns the 257th key and the epilogue.
-    const int R = (warp - 1) >> 3;           // 0: warps 1-8, 1: warps 9-16
-    const int hf = ((warp - 1) >> 2) & 1;
-    const int quad = warp & 3;               // TMEM lane quadrant is fixed by the hardware warp id
-    const int r = quad * 32 + lane;
-    const uint32_t lane_addr = uint32_t(quad * 32) << 16;
-    const uint32_t treg = tmem_base + R * 256 + lane_addr;
-    uint32_t s_ph = 0, o_ph = 0, q_ph = 0;
-    long long g_sf = 0, g_of = 0, g_bar = 0; const long long g_begin = clock64();
-    uint8_t* sP = smem + C::OFF_P + R * C::P_BYTES;
-    const uint8_t* sQ = smem + C::OFF_Q + R * C::Q_BYTES;
-    __nv_bfloat16* xmax = reinterpret_cast<__nv_bfloat16*>(smem + C::OFF_XMAX) + R * 256;   // [2 halves][128]
-    float* xsum = reinterpret_cast<float*>(smem + C::OFF_XSUM) + R * 128;                    // [128] (written by half 1)
-    for (int g = R; g < n_tiles; g += 2) {
-      const int qt = g % TPI, it = g / TPI, item = (int)blockIdx.x + it * (int)gridDim.x;
-      const int f = item / p.heads, h = item % p.heads;
-      const int qrow = qt * 128 + r;
-      const bool warp_active = (qt * 128 + quad * 32) < p.tokens;
-      const __nv_bfloat16* kx = reinterpret_cast<const __nv_bfloat16*>(smem + C::OFF_X + R * 384);
-      const __nv_bfloat16* vx = kx + 64 + ((g >> 1) & 1) * 64;
-      __syncwarp();
-      const long long ts_ = clock64();
-      mbar_wait(&q_full[R], q_ph);           // Q tile and the extra key/value row of this tile are in shared memory
-      q_ph ^= 1;
-      mbar_wait(&s_full[R], s_ph);
-      g_sf += clock64() - ts_;
-      s_ph ^= 1;
-      tc_fence_after();
-      float mx = -INFINITY, s_x = 0.f;
-      if (warp_active) {
-        if (hf == 0) {
-          // score against the 257th key on CUDA cores: q row from the swizzled Q tile
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const uint4 qv = *reinterpret_cast<const uint4*>(sQ + r * 128 + ((j ^ (r & 7)) << 4));
-            const uint4 kv = *reinterpret_cast<const uint4*>(kx + j * 8);
-            s_x += bf16_lo(qv.x) * bf16_lo(kv.x) + bf16_hi(qv.x) * bf16_hi(kv.x) + bf16_lo(qv.y) * bf16_lo(kv.y) + bf16_hi(qv.y) * bf16_hi(kv.y) +
-                   bf16_lo(qv.z) * bf16_lo(kv.z) + bf16_hi(qv.z) * bf16_hi(kv.z) + bf16_lo(qv.w) * bf16_lo(kv.w) + bf16_hi(qv.w) * bf16_hi(kv.w);
-          }
-          mx = s_x;
-        }
-        // TMEM loads are asynchronous until tcgen05.wait::ld: keep the NEXT 32-column chunk in flight while the
-        // current one is processed (two register buffers), instead of paying the TMEM round trip per chunk
-        uint32_t va[32], vb[32];
-        tmem_ld_32x32(treg + hf * 128, va);
-#pragma unroll
-        for (int c = 0; c < 4; c += 2) {
-          tmem_ld_wait();
-          tmem_ld_32x32(treg + hf * 128 + (c + 1) * 32, vb);
-#pragma unroll
-          for (int i = 0; i < 32; ++i) mx = fmaxf(mx, __uint_as_float(va[i]));
-          tmem_ld_wait();
-          if (c + 2 < 4) tmem_ld_32x32(treg + hf * 128 + (c + 2) * 32, va);
-#pragma unroll
-          for (int i = 0; i < 32; ++i) mx = fmaxf(mx, __uint_as_float(vb[i]));
-        }
-      }
-      // both halves must subtract the SAME offset: each rounds its own max to bf16 and takes the max of the two rounded
-      // values (any common offset within a few % of the true max is numerically fine; the sums use it consistently)
-      const __nv_bfloat16 mxb = __float2bfloat16_rn(mx);
-      xmax[hf * 128 + r] = mxb;
-      { const long long tb_ = clock64(); asm volatile("bar.sync %0, 256;" ::"r"(1 + R) : "memory"); g_bar += clock64() - tb_; }
-      float part = 0.f, p_x = 0.f;
-      if (warp_active) {
-        mx = fmaxf(__bfloat162float(mxb), __bfloat162float(xmax[(hf ^ 1) * 128 + r]));
-        const float mb = mx * p.scale_log2e;
-        auto exp_store = [&](const uint32_t (&v)[32], int c) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            float e[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              e[i] = fast_exp2(fmaf(__uint_as_float(v[8 * j + i]), p.scale_log2e, -mb));
-              part += e[i];
-            }
-            st_sw128_row16(sP, 128, r, hf * 128 + c * 32 + j * 8,
-                           make_uint4(pack_bf16x2(e[0], e[1]), pack_bf16x2(e[2], e[3]), pack_bf16x2(e[4], e[5]), pack_bf16x2(e[6], e[7])));
-          }
-        };
-        uint32_t va[32], vb[32];
-        tmem_ld_32x32(treg + hf * 128, va);
-#pragma unroll
-        for (int c = 0; c < 4; c += 2) {
-          tmem_ld_wait();
-          tmem_ld_32x32(treg + hf * 128 + (c + 1) * 32, vb);
-          exp_store(va, c);
-          tmem_ld_wait();
-          if (c + 2 < 4) tmem_ld_32x32(treg + hf * 128 + (c + 2) * 32, va);
-          exp_store(vb, c + 1);
-        }
-        if (hf == 0) {
-          p_x = fast_exp2(fmaf(s_x, p.scale_log2e, -mb));
-          part += p_x;
-        } else {
-          xsum[r] = part;
-        }
-      } else {
-        for (int col = 0; col < 128; col += 8) st_sw128_row16(sP, 128, r, hf * 128 + col, make_uint4(0, 0, 0, 0));
-      }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(&p_full[R]);               // (release) also publishes xsum to half 0: p_full -> T0 -> o_full -> half 0
-
-      if (hf == 0) {
-        __syncwarp();
-        { const long long to_ = clock64(); mbar_wait(&o_full[R], o_ph); g_of += clock64() - to_; }
-        o_ph ^= 1;
-        tc_fence_after();
-        if (warp_active) {
-          const float inv = __frcp_rn(part + xsum[r]);
-          __nv_bfloat16* dst = p.ctx + ((size_t)f * p.tokens + qrow) * p.D + h * 64;
-          uint32_t vo[2][32];
-          tmem_ld_32x32(treg + C::O_OFF, vo[0]);
-          tmem_ld_32x32(treg + C::O_OFF + 32, vo[1]);
-          tmem_ld_wait();
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            const uint32_t (&v)[32] = vo[c];
-            if (qrow < p.tokens) {
-              float o[32];
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const uint4 vv = *reinterpret_cast<const uint4*>(vx + c * 32 + j * 8);
-                const float xv[8] = {bf16_lo(vv.x), bf16_hi(vv.x), bf16_lo(vv.y), bf16_hi(vv.y), bf16_lo(vv.z), bf16_hi(vv.z), bf16_lo(vv.w), bf16_hi(vv.w)};
-#pragma unroll
-                for (int e = 0; e < 8; ++e) o[j * 8 + e] = fmaf(p_x, xv[e], __uint_as_float(v[j * 8 + e])) * inv;
-              }
-              uint4* op = reinterpret_cast<uint4*>(dst + c * 32);
-#pragma unroll
-              for (int j = 0; j < 4; ++j)
-                op[j] = make_uint4(pack_bf16x2(o[8 * j], o[8 * j + 1]), pack_bf16x2(o[8 * j + 2], o[8 * j + 3]),
-                                   pack_bf16x2(o[8 * j + 4], o[8 * j + 5]), pack_bf16x2(o[8 * j + 6], o[8 * j + 7]));
-            }
-          }
-        }
-        __syncwarp();
-        tc_fence_before();
-        mbar_arrive(&r_free[R]);
-      }
-    }
-    if (p.dbg && hf == 0 && r == 0) { long long* o = p.dbg + (size_t)blockIdx.x * 16 + 8 + R * 4; o[0] = clock64() - g_begin; o[1] = g_sf; o[2] = g_bar; o[3] = g_of; }
-  } else {
-    // ================= warp 17: query row 256 (the last token) of every item, on CUDA cores =================
-    // scores: lane l owns keys l + 32 i (i = 0..7) and the whole q row in registers; P V: half-warp hw owns keys 2 t + hw, lane
-    // (hl) owns head dims 4 hl .. 4 hl + 3.  fp32 throughout (the tile path rounds P to bf16 for the MMA).
-    pdl_wait();
-    const int hl = lane & 15, hw = lane >> 4;
-    const uint8_t* sK = smem + C::OFF_K;
-    const uint8_t* sV = smem + C::OFF_V;
-    uint32_t kf_ph = 0, vf_ph = 0;
-    for (int it = 0; it < my_items; ++it) {
-      const int item = (int)blockIdx.x + it * (int)gridDim.x;
-      const int f = item / p.heads, h = item % p.heads;
-      const __nv_bfloat16* xrow = p.qkv + ((size_t)f * p.tokens + 256) * (3 * (size_t)p.D) + h * 64;
-      uint4 qw[8];
-#pragma unroll
-      for (int c = 0; c < 8; ++c) qw[c] = __ldg(reinterpret_cast<const uint4*>(xrow) + c);
-      auto dot8 = [](const uint4 a, const uint4 b) {
-        return bf16_lo(a.x) * bf16_lo(b.x) + bf16_hi(a.x) * bf16_hi(b.x) + bf16_lo(a.y) * bf16_lo(b.y) + bf16_hi(a.y) * bf16_hi(b.y) +
-               bf16_lo(a.z) * bf16_lo(b.z) + bf16_hi(a.z) * bf16_hi(b.z) + bf16_lo(a.w) * bf16_lo(b.w) + bf16_hi(a.w) * bf16_hi(b.w);
-      };
-      float s_x = 0.f;
-#pragma unroll
-      for (int c = 0; c < 8; ++c) s_x += dot8(qw[c], __ldg(reinterpret_cast<const uint4*>(xrow + p.D) + c));
-      const uint2 vxw = __ldg(reinterpret_cast<const uint2*>(xrow + 2 * p.D) + hl);
-      mbar_wait(k_full, kf_ph);
-      kf_ph ^= 1;
-      float sc[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int row = lane + 32 * i;
-        const uint8_t* kr = sK + (row >> 7) * (128 * 128) + (row & 127) * 128;
-        float a = 0.f;
-#pragma unroll
-        for (int c = 0; c < 8; ++c) a += dot8(qw[c], *reinterpret_cast<const uint4*>(kr + ((c ^ (row & 7)) << 4)));
-        sc[i] = a;
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(k_done);            // K may be refilled (together with the last S-MMA's commit)
-      float mx = s_x;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) mx = fmaxf(mx, sc[i]);
-      mx = warp_max(mx);
-      const float mb = mx * p.scale_log2e;
-      float part = 0.f;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        sc[i] = fast_exp2(fmaf(sc[i], p.scale_log2e, -mb));
-        part += sc[i];
-      }
-      const float p_x = fast_exp2(fmaf(s_x, p.scale_log2e, -mb));
-      const float inv = __frcp_rn(warp_sum(part) + p_x);
-      mbar_wait(v_full, vf_ph);
-      vf_ph ^= 1;
-      float o0 = 0.f, o1 = 0.f, o2 = 0.f, o3 = 0.f;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-#pragma unroll 8
-        for (int t = 0; t < 16; ++t) {
-          const int j = 32 * i + 2 * t + hw;           // key; its weight sits in sc[i] of lane j & 31
-          const float pj = __shfl_sync(0xffffffffu, sc[i], 2 * t + hw);
-          const uint8_t* vr = sV + (j >> 7) * (128 * 128) + (j & 127) * 128;
-          const uint2 w = *reinterpret_cast<const uint2*>(vr + ((((hl >> 1) ^ (j & 7)) << 4) | ((hl & 1) << 3)));
-          o0 = fmaf(pj, bf16_lo(w.x), o0); o1 = fmaf(pj, bf16_hi(w.x), o1);
-          o2 = fmaf(pj, bf16_lo(w.y), o2); o3 = fmaf(pj, bf16_hi(w.y), o3);
-        }
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(v_done);            // V may be refilled (together with the last P V's commit)
-      o0 += __shfl_xor_sync(0xffffffffu, o0, 16); o1 += __shfl_xor_sync(0xffffffffu, o1, 16);
-      o2 += __shfl_xor_sync(0xffffffffu, o2, 16); o3 += __shfl_xor_sync(0xffffffffu, o3, 16);
-      if (hw == 0) {
-        o0 = fmaf(p_x, bf16_lo(vxw.x), o0) * inv; o1 = fmaf(p_x, bf16_hi(vxw.x), o1) * inv;
-        o2 = fmaf(p_x, bf16_lo(vxw.y), o2) * inv; o3 = fmaf(p_x, bf16_hi(vxw.y), o3) * inv;
-        *reinterpret_cast<uint2*>(p.ctx + ((size_t)f * p.tokens + 256) * p.D + h * 64 + hl * 4) = make_uint2(pack_bf16x2(o0, o1), pack_bf16x2(o2, o3));
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, C::TMEM_COLS);
-  }
+  const uint32_t* kbits = p.key_bits ? p.key_bits + (size_t)b * p.mask_words : nullptr;
+  const int q_pos0 = p.past + qt * 64;                       // absolute position of tile row 0
+  flash_attention_tile<128>(
+      smem, base_u32, q_full, kv_full, nkv, p.scale_log2e, load_kv,
+      [&](int r, int key) {
+        return key <= q_pos0 + r && key < kv_len && (kbits == nullptr || ((__ldg(kbits + (key >> 5)) >> (key & 31)) & 1u));
+      },
+      [&](int r, int col, float o0, float o1) {
+        const int q = qt * 64 + r;
+        if (q < p.S) *reinterpret_cast<uint32_t*>(p.ctx + ((size_t)b * p.S + q) * p.H + h * 128 + col) = pack_bf16x2(o0, o1);
+      });
 }
 
 }  // namespace vly

@@ -1,9 +1,6 @@
-// Shared device-side primitives for the sm_100a kernels: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (TMEM alloc / mma / commit / ld), UMMA shared-memory + instruction descriptors.
-// Hand-written inline PTX; no CUTLASS/CuTe.  Bit layouts follow the PTX ISA "tcgen05" chapter
-// (matrix descriptor: start[0,14) LBO[16,30) SBO[32,46) version[46,48)=1 layout[61,64);
-//  instruction descriptor: c_format[4,6) a_format[7,10) b_format[10,13) a_major[15] b_major[16]
-//  n>>3 [17,23) m>>4 [24,29)).
+// Shared device-side primitives for the sm_90a kernels: mbarrier, TMA (cp.async.bulk.tensor), the wgmma
+// shared-memory matrix descriptor.  Hand-written inline PTX; no CUTLASS/CuTe.  Bit layouts follow the PTX ISA
+// "Asynchronous Warpgroup Level Matrix" chapter.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -15,22 +12,10 @@
 
 namespace vly {
 
-constexpr int kNumSMsDefault = 148;
-
 // ------------------------------------------------------------------------------------------
 // misc
 // ------------------------------------------------------------------------------------------
 VLY_DEVINL uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-
-VLY_DEVINL bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.b32 %0, 1, 0, P;\n\t}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
 
 VLY_DEVINL uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
@@ -47,7 +32,6 @@ VLY_DEVINL void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(smem_u32(bar)), "r"(count));
 }
 VLY_DEVINL void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory"); }
-VLY_DEVINL void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 
 VLY_DEVINL void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
@@ -85,19 +69,6 @@ VLY_DEVINL void tma_load_2d(void* smem_dst, const CUtensorMap* m, uint64_t* bar,
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-// 2D tile store (shared -> global, bulk async-group completion): out-of-bounds rows / columns of the box are not written.
-// The generic-proxy writes that filled the tile must be followed by fence.proxy.async.shared::cta in the writing threads.
-VLY_DEVINL void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];\n" ::"l"(reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-               : "memory");
-}
-VLY_DEVINL void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;\n" ::: "memory"); }
-template <int N>
-VLY_DEVINL void bulk_wait_group_read() {      // at most N of this thread's bulk groups still READ their shared-memory source
-  asm volatile("cp.async.bulk.wait_group.read %0;\n" ::"n"(N) : "memory");
-}
-VLY_DEVINL void bulk_wait_group_all() { asm volatile("cp.async.bulk.wait_group 0;\n" ::: "memory"); }
 VLY_DEVINL void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];\n" ::"r"(
@@ -118,127 +89,22 @@ VLY_DEVINL void pdl_wait() { asm volatile("griddepcontrol.wait;\n" ::: "memory")
 VLY_DEVINL void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;\n" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, fences, commit, mma, ld
-// ------------------------------------------------------------------------------------------
-VLY_DEVINL void tmem_alloc(uint32_t* smem_slot, uint32_t ncols) {  // whole warp, ncols pow2 >= 32
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_slot)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
-VLY_DEVINL void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp (the allocating one)
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols) : "memory");
-}
-VLY_DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-VLY_DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
-
-// MMA-completion -> mbarrier arrive (implicitly fence::before_thread_sync).
-VLY_DEVINL void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// D[tmem] (+)= A[smem] * B[smem]; bf16 inputs, fp32 accumulate.  Issued by ONE thread.
-VLY_DEVINL void tc_mma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// ---- cta_group::2 (CTA pair) variants: one MMA spans two SMs (M = 256); the leader CTA (rank 0) issues it ----
-VLY_DEVINL uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(r));
-  return r;
-}
-VLY_DEVINL void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;\n" ::: "memory");
-}
-VLY_DEVINL void tmem_alloc_cg2(uint32_t* smem_slot, uint32_t ncols) {   // one warp in EACH CTA of the pair, same slot offset
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_slot)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;\n" ::: "memory");
-}
-VLY_DEVINL void tmem_dealloc_cg2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols) : "memory");
-}
-VLY_DEVINL void tc_mma_bf16_cg2(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// MMA-completion -> arrive on the same-offset mbarrier of BOTH CTAs of the pair
-VLY_DEVINL void tc_commit_cg2(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n" ::"r"(smem_u32(bar)),
-               "h"((uint16_t)3)
-               : "memory");
-}
-// 2-SM TMA load: data lands in THIS CTA's shared memory, the transaction bytes are credited to the LEADER's mbarrier
-// (same offset, CTA-rank bit 24 of the shared::cluster address cleared)
-VLY_DEVINL void tma_load_2d_cg2(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];\n" ::"r"(
-          smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-      : "memory");
-}
-// arrive on the mbarrier at the same offset in CTA `rank` of the cluster
-VLY_DEVINL void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
-  uint32_t ra;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;\n" : "=r"(ra) : "r"(smem_u32(bar)), "r"(rank));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];\n" ::"r"(ra) : "memory");
-}
-
-// Instruction descriptor for kind::f16 with BF16 A/B, FP32 D.  b_mn_major=1 -> B is MN-major.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major = 0, int b_mn_major = 0) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (uint32_t(a_mn_major) << 15) | (uint32_t(b_mn_major) << 16) |
-         (uint32_t(N >> 3) << 17) | (uint32_t(M >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor, 128-byte swizzle.
+// wgmma shared-memory matrix descriptor (sm_90a), 128-byte swizzle:
+//  start[0,14) LBO[16,30) SBO[32,46) (all in 16-byte units), base_offset[49,52) = 0 (1024-byte aligned atoms),
+//  layout[62,64) = 1 (SWIZZLE_128B).
 //  K-major operand : rows of 128 B (64 bf16 of K), 8-row atoms of 1024 B;  SBO = 1024 (next 8 rows), LBO unused.
 //  MN-major operand: "rows" are K-slices of 128 B (64 bf16 of M/N), 8 of them per 1024 B atom;
 //                    SBO = 1024 (next 8 K), LBO = byte distance between 64-element M/N chunks.
+// Advancing K by 16 elements inside a K-major atom is +32 B, i.e. +2 in the start field.
+// ------------------------------------------------------------------------------------------
 VLY_DEVINL uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= uint64_t((smem_addr >> 4) & 0x3FFF);
   d |= uint64_t((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= uint64_t((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= uint64_t(1) << 46;  // descriptor version (Blackwell)
-  d |= uint64_t(2) << 61;  // SWIZZLE_128B
+  d |= uint64_t(1) << 62;  // SWIZZLE_128B
   return d;
 }
-
-// TMEM -> registers: this warp's 32 lanes (its quadrant), 32 consecutive fp32 columns.
-// taddr = (lane_base << 16) | column, lane_base = 32 * (warp_idx % 4).
-VLY_DEVINL void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-VLY_DEVINL void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-VLY_DEVINL void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------
 // vector global access
@@ -249,9 +115,6 @@ VLY_DEVINL uint4 ldg_nc_v4(const void* p) {
                : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
                : "l"(p));
   return r;
-}
-VLY_DEVINL void stg_v4(void* p, uint4 v) {
-  asm volatile("st.global.v4.u32 [%0], {%1, %2, %3, %4};\n" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
 
 VLY_DEVINL float fast_exp2(float x) {  // MUFU.EX2; exp2(-inf) = 0

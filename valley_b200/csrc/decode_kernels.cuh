@@ -1,4 +1,4 @@
-// Decode path, generation 2: HBM-bound weight streaming done the Blackwell way.
+// Decode path, generation 2: HBM-bound weight streaming with TMA bulk copies and mbarriers.
 //
 //   gemv_ring_kernel : y[b,n] = sum_k x[b,k] W[n,k] for B <= 4.  One persistent CTA per SM.  A producer warp streams the
 //                      weight rows through a shared-memory ring with 1-D bulk (TMA) copies -- 8 rows x 2048 columns (32 KB)
@@ -19,7 +19,7 @@
 namespace vly {
 
 struct RingCfg {
-  static constexpr int ROWS = 4;                          // rows per work unit: N/4 units balance to ~1% over 148 SMs
+  static constexpr int ROWS = 4;                          // rows per work unit: N/4 units balance to ~1% over the SMs
   static constexpr int KC = 2048;                         // columns per slice
   static constexpr int STAGE_BYTES = ROWS * KC * 2;       // 16 KB
   static constexpr int THREADS = 288;                     // warp 0 = producer, warps 1..8 = consumers

@@ -9,8 +9,8 @@
 //                       activations -- so while the consumers sit in a grid barrier the ring fills with the NEXT phase's
 //                       weights and HBM keeps streaming.  The ring geometry is PER PHASE (PhaseDesc::rows, ::kc, chosen on the
 //                       host per matrix shape): K is cut into equal stages (no short tail stage: 5120 = 2 x 2560, not
-//                       2048 + 2048 + 1024) and the rows per work unit are picked so the units balance over the 148 SMs
-//                       (5120 rows = 640 units of 8 = 4.3 per SM -> 5 rounds at 86 %; 1280 units of 4 -> 9 rounds at 96 %).
+//                       2048 + 2048 + 1024) and the rows per work unit are picked so the units balance over the SMs
+//                       (on 132 SMs: 5120 rows = 640 units of 8 = 4.8 per SM -> 5 rounds at 97 %; 1280 units of 4 -> 10 rounds at 97 %).
 //   warps 1..16       : compute -- per phase: the activation rows arrive in shared memory by bulk copy (RMSNorm statistics
 //                       where a norm is folded), multiply the ring stages (fp32 accumulate), warp-reduce, and hand the 16
 //                       per-warp partials of a work unit to the finalize warp through a 4-slot mbarrier handoff -- there is NO
@@ -29,22 +29,11 @@
 namespace vly {
 
 enum PhaseType : int { PH_QKV = 0, PH_ATTN = 1, PH_OPROJ = 2, PH_GATEUP = 3, PH_DOWN = 4, PH_LOGITS = 5 };
-enum PhaseFlags : int { PHF_FIRST = 1, PHF_LAST = 2, PHF_LOCAL_SYNC = 4, PHF_NO_SYNC = 8 };
 
 struct PhaseDesc {
   int type, N, K, layer;
   int rows, kc;                 // ring geometry of this phase: weight rows per work unit, columns per ring stage
   int inflight;                 // stages of THIS phase's size kept in flight (~100 KB of bulk copies outstanding per SM)
-  // tcgen05 consumer (decode_umma.cuh) only: a weight matrix whose K does not fit the activation block is walked in sub-phases
-  int k_off;                    // first column of this (sub-)phase in the rows of W and of x_in
-  int ldx;                      // row stride of x_in in elements (the matrix's full K)
-  int x_cols;                   // columns of x_in staged at the start of this phase (0: the block staged by the previous sub-phase is reused)
-  int x_panel0;                 // 64-column panel of the staged block that holds column k_off
-  int flags;                    // PHF_FIRST: accumulators start from zero; PHF_LAST: the epilogue runs; PHF_LOCAL_SYNC: only this
-                                // CTA synchronises after it (the next sub-phase re-stages x), no grid barrier; PHF_NO_SYNC: none at all
-  int pad_;
-  const void* tmap;             // CUtensorMap of W: dims {64, N, K/64}, box {64, 8, kc/64}
-  const void* xmap;             // CUtensorMap of x_in (8 rows tall, rows >= B zero): dims {64, 8, K/64}, box {64, 8, x_cols/64}
   const __nv_bfloat16* W;       // [N, K] (nullptr for PH_ATTN)
   const __nv_bfloat16* x_in;    // activation rows [B, K]
   __nv_bfloat16* out;           // QKV: q [B,H]; OPROJ/DOWN: x [B,H] (in place, also the residual); GATEUP: hb [B,I]
@@ -151,11 +140,9 @@ VLY_DEVINL void mega_attention_phase(const StepParams& p, const PhaseDesc& d, co
   // tree (8 instead of 32 shuffles), softmax runs online in registers across the passes of an item, P.V accumulates per
   // lane over its 8 head dims.  Items are dealt warp-major over the SMs so one layer's K/V is pulled by every SM at once.
   const int len = pos + 1;
-  // Item size = a multiple of 16 keys (one 16-key pass per 16).  Measured at B = 4, 40 heads (profiles/decode_ab_r02.txt, calls 25-26):
-  // what costs is the NUMBER of items -- every item ends in a publish (partial stores, fence, atomic) and is one more partial
-  // for the merge, ~8 us of shared-resource time per "round" of 2368 items -- while a pass adds ~3 us to a warp's serial chain:
-  //   461 keys: 2400 32-key items 23 us | 4640 16-key items 30 us;   591 keys: 2080 48-key items 26 us | 5920 16-key items 48 us.
-  // So: 16 keys if every 16-key item finds its own warp (B = 1), else the smallest multiple of 16 >= 32 whose item count fits the
+  // Item size = a multiple of 16 keys (one 16-key pass per 16).  What costs is the NUMBER of items -- every item ends in a
+  // publish (partial stores, fence, atomic) and is one more partial for the merge -- while a pass only lengthens a warp's serial
+  // chain.  So: 16 keys if every 16-key item finds its own warp (B = 1), else the smallest multiple of 16 >= 32 whose item count fits the
   // warps (5 % overflow into a second, nearly empty round costs less than a third pass for everybody).
   const int n_warps = 16 * (int)gridDim.x;
   int ikeys = p.attn_ikeys;
@@ -477,7 +464,7 @@ __global__ void __launch_bounds__(576, 1) decode_step_kernel(const StepParams p)
       int st = 0;
       uint32_t ph = 0;
       // The ring may be deeper than the number of copies kept in flight: what streams fastest is a bounded number of bytes
-      // outstanding per SM (tools/ringbw.cu), but while the consumers sit in a grid barrier / stage activations the extra
+      // outstanding per SM, but while the consumers sit in a grid barrier / stage activations the extra
       // slots keep HBM busy.
       int wst = 0, issued = 0, confirmed = 0;
       uint32_t wph = 0;
@@ -631,8 +618,8 @@ __global__ void __launch_bounds__(576, 1) decode_step_kernel(const StepParams p)
             // W[g][k..k+7]; both operands use the same k permutation, so two MMAs consume them.  The 32-wide k blocks of a
             // stage are dealt round-robin to the 16 warps.
             const int gq = lane >> 2, tq = lane & 3;
-            // (the legacy HMMA pipe of this part sustains ~1 m16n8k16 per 40 cycles per SM sub-partition -- tools/ringbw.cu -- so
-            //  the consumers, not HBM, bound this path; two accumulators keep the pair of MMAs of a k block independent)
+            // (two accumulators keep the pair of MMAs of a k block independent: the MMA latency, not the issue rate, would
+            //  otherwise bound the consumers)
             float dacc[4] = {0.f, 0.f, 0.f, 0.f}, dacc1[4] = {0.f, 0.f, 0.f, 0.f};
             const bool w_ok = gq < rows, x_ok = gq < p.B;
             for (int s = 0; s < n_slices; ++s) {

@@ -1,17 +1,13 @@
-// Persistent, warp-specialised tcgen05 GEMM:  D[M,N] = A[M,K] * B[N,K]^T   (bf16 in, fp32 accumulate in TMEM)
+// Warp-specialised Hopper GEMM:  D[M,N] = A[M,K] * B[N,K]^T   (bf16 in, fp32 accumulate in registers)
 //
-//   warp 0      : TMA producer  (A tile 128x64, B tile BNx64 per stage, 128B swizzle, mbarrier complete_tx)
-//   warp 1      : TMEM allocator + single-thread tcgen05.mma issuer (UMMA 128 x BN x 16), tcgen05.commit
-//   warps 2..5  : epilogue -- tcgen05.ld the accumulator (one TMEM lane == one output row per thread),
-//                 apply the fused epilogue, store.  Two accumulator stages in TMEM so the epilogue
-//                 of tile i overlaps the main loop of tile i+1.
-//   TEPI = true : the bf16 output leaves through shared memory and TMA tensor stores, and the residual rows arrive by TMA loads:
-//                 a thread owns a ROW of the tile, so its 16-byte global stores / loads touched 32 different 128-byte lines per
-//                 warp instruction -- 32 LSU cycles each, ~4000 cycles per 128 x 256 tile for the stores alone, as long as the
-//                 main loop of a K = 1024 tile (ncu: tensor pipe 45-62 % active on the ViT's QKV / fc1 / out_proj GEMMs; more
-//                 epilogue warps made it worse).  Each epilogue warp stages 32 rows x 64 columns (4 KB, 128-byte swizzle:
-//                 conflict-free 16-byte shared stores) and one lane issues a cp.async.bulk.tensor store of the box; tile edges are
-//                 clipped by the TMA unit.
+//   warpgroup 0    : TMA producer (one thread): A tile 128x64, B tile BNx64 per stage, 128B swizzle, mbarrier complete_tx
+//   warpgroups 1-2 : consumers -- each owns 64 rows of the 128-row tile and issues wgmma.mma_async m64n128k16 (BN / 128 per
+//                    k-step) straight from the shared-memory ring; one wgmma group stays in flight while the previous stage
+//                    is handed back to the producer.
+//   epilogue       : the accumulators go through shared memory (the ring is free once the main loop has drained) so that
+//                    every thread owns 32-column chunks of ONE output row -- the row statistics, RoPE pairs and SwiGLU pairs
+//                    below are row-local -- then the fused epilogue is applied and the row is stored.
+//   One 128 x BN tile per CTA: the grid covers the tiles.
 //
 // Both operands are K-major, i.e. A is a row-major activation matrix and B is an nn.Linear weight
 // [out_features, in_features] exactly as HuggingFace stores it.
@@ -24,6 +20,7 @@
 //   bias, quick_gelu, residual add, SwiGLU (gate/up rows interleaved), RoPE + KV-cache append.
 #pragma once
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace vly {
 
@@ -66,19 +63,6 @@ struct GemmParams {
   long long peer_frame_off;
 };
 
-template <int BN>
-struct GemmCfg {
-  static constexpr int BM = 128, BK = 64;
-  static constexpr int STAGES = (BN == 256) ? 4 : 6;
-  static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = BN * BK * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int TMEM_COLS = 2 * BN;                        // 2 accumulator stages (256 or 512)
-  static constexpr int VEC_BYTES = 2 /*acc stages*/ * 2 /*bias, colsum*/ * BN * 4;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + VEC_BYTES;
-  static constexpr int THREADS = 192;
-};
-
 // x*sigmoid(1.702x) and x*sigmoid(x) on the fast MUFU path (ex2.approx + rcp.approx)
 // sigmoid(y) = 0.5 + 0.5 tanh(y / 2): ONE MUFU op (tanh.approx.f32, |rel err| ~ 2^-11, far below the bf16 rounding of the result)
 // instead of two (ex2 + rcp).  A 128 x 256 fc1 tile has 32768 activations per CTA: at 16 MUFU ops per clock per SM the
@@ -97,535 +81,319 @@ VLY_DEVINL float silu_f(float v) {         // v * sigmoid(v)
   return fmaf(h, tanh_approx(h), h);
 }
 
-// shared-memory footprint of a launch (TEPI: 5 ring stages of 32 KB + 4 warps x 3 staging boxes of 4 KB)
-template <int BN, bool TEPI>
-constexpr int gemm_smem_bytes() {
-  return TEPI ? 5 * 32768 + 4 * 3 * 4096 + 1024 + 256 + GemmCfg<BN>::VEC_BYTES : GemmCfg<BN>::SMEM_BYTES;
-}
+template <int BN>
+struct GemmCfg {
+  static_assert(BN == 128 || BN == 256, "tile width");
+  static constexpr int BM = 128, BK = 64;
+  static constexpr int STAGES = (BN == 256) ? 4 : 6;
+  static constexpr int A_BYTES = BM * BK * 2;
+  static constexpr int B_BYTES = BN * BK * 2;
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int RING_BYTES = STAGES * STAGE_BYTES;               // 192 KB
+  static constexpr int ACC_LD = BN + 4;                                 // fp32 staging row pitch (floats)
+  static_assert(BM * ACC_LD * 4 <= RING_BYTES, "accumulator staging must fit in the drained ring");
+  static constexpr int VEC_BYTES = 2 /*bias, colsum*/ * BN * 4;
+  static constexpr int SMEM_BYTES = RING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + VEC_BYTES;
+  static constexpr int THREADS = 384;
+};
 
-// CG2 = true: launched as clusters of 2 CTAs; the pair computes a 256 x BN tile with cta_group::2 MMAs (each CTA holds
-// 128 rows of A and BN/2 rows of B per stage and ends up with its own 128 output rows in its own TMEM).
-template <int BN, int EPI, bool CG2 = false, bool TEPI = false>
-__global__ void __launch_bounds__(192, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const __grid_constant__ CUtensorMap tma_o,
-               const __grid_constant__ CUtensorMap tma_r, const GemmParams p) {
-  static_assert(!TEPI || ((BN == 128 || CG2) && (EPI == EPI_BIAS || EPI == EPI_LN_BIAS || EPI == EPI_LN_BIAS_GELU || EPI == EPI_BIAS_RES_STATS ||
-                                                 EPI == EPI_RMS_SWIGLU)),
-                "TMA-store epilogue: 32 KB stages and a bf16 row-major output only");
+template <int BN, int EPI>
+__global__ void __launch_bounds__(384, 1)
+gemm_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b, const GemmParams p) {
   using Cfg = GemmCfg<BN>;
-  constexpr int BM = Cfg::BM, BK = Cfg::BK;
-  constexpr int B_ROWS = CG2 ? BN / 2 : BN;                      // rows of B this CTA stages
-  constexpr int B_BYTES = B_ROWS * BK * 2;
-  constexpr int STAGE_BYTES = Cfg::A_BYTES + B_BYTES;
-  constexpr int STAGES = TEPI ? 5 : (CG2 ? 6 : Cfg::STAGES);     // 32 KB stages in pair mode
-  static_assert(STAGES * STAGE_BYTES <= Cfg::STAGES * Cfg::STAGE_BYTES, "pair-mode ring must fit the single-CTA budget");
-  constexpr int STG_BOX = 4096;                                  // staging box: 32 rows x 64 bf16 columns
-  constexpr int RING_END = TEPI ? STAGES * STAGE_BYTES + 4 * 3 * STG_BOX : Cfg::STAGES * Cfg::STAGE_BYTES;
+  constexpr int BM = Cfg::BM, BK = Cfg::BK, STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base_u32 = (smem_u32(smem_raw) + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (base_u32 - smem_u32(smem_raw));
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * Cfg::A_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + RING_END);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::RING_BYTES);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* tmem_full = bars + 2 * STAGES;
-  uint64_t* tmem_empty = bars + 2 * STAGES + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-  uint64_t* res_full_all = bars + 2 * STAGES + 5;                 // [4 epilogue warps][2]: residual boxes have landed (TEPI)
-  float* svec = reinterpret_cast<float*>(smem + RING_END + 256);   // [2][2][BN]
+  float* sbias = reinterpret_cast<float*>(smem + Cfg::RING_BYTES + 256);   // [BN]
+  float* scol = sbias + BN;                                                  // [BN]
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
   const int num_kb = (p.K + BK - 1) / BK;
-  // work distribution: single CTA -> one 128-row tile per step; pair -> one 256-row tile per step, this CTA owns half
-  const uint32_t cta_rank = CG2 ? cluster_ctarank() : 0;
-  const int num_workers = CG2 ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  const int worker = CG2 ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int num_m_steps = CG2 ? (p.num_m_tiles + 1) / 2 : p.num_m_tiles;
-  const int num_tiles = num_m_steps * p.num_n_tiles;
+  const int m_blk = (int)blockIdx.x / p.num_n_tiles, n_blk = (int)blockIdx.x % p.num_n_tiles;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tma_a);
     tma_prefetch_desc(&tma_b);
-    if constexpr (TEPI) {
-      tma_prefetch_desc(&tma_o);
-      if constexpr (EPI == EPI_BIAS_RES_STATS) tma_prefetch_desc(&tma_r);
-      for (int i = 0; i < 8; ++i) mbar_init(&res_full_all[i], 1);
-    }
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], CG2 ? 256 : 128);               // pair mode: both CTAs' epilogues release the leader's accumulator
+      mbar_init(&empty_bar[i], 256);                             // every consumer thread releases the stage
     }
     fence_barrier_init();
   }
-  if constexpr (CG2) cluster_sync_all();                         // peer barriers are initialised before anyone signals them
-  if (warp == 1) {
-    if constexpr (CG2) tmem_alloc_cg2(tmem_slot, Cfg::TMEM_COLS);
-    else tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // Programmatic dependent launch: everything above (barrier init, TMEM allocation, descriptor prefetch) touches nothing the
-  // previous kernel of the stream produces, so when the launch carries the programmatic-serialisation attribute it overlaps that
-  // kernel's tail; the threads that read or overwrite its data (TMA producer, epilogue) wait for its completion first.
+  // Programmatic dependent launch: the prologue above touches nothing the previous kernel of the stream produces, so under the
+  // programmatic-serialisation attribute it overlaps that kernel's tail; the threads that read its data wait for it first.
   pdl_launch_dependents();
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================================== TMA producer =====================================
-    if (lane == 0) {
+    if (threadIdx.x == 0) {
       pdl_wait();
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = worker; tile < num_tiles; tile += num_workers) {
-        const int m_step = tile / p.num_n_tiles, n_blk = tile % p.num_n_tiles;
-        const int m_blk = CG2 ? 2 * m_step + (int)cta_rank : m_step;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          if constexpr (CG2) {
-            // both CTAs' bytes are credited to the LEADER's full barrier; only the leader arms it
-            if (cta_rank == 0) mbar_expect_tx(&full_bar[stage], 2 * STAGE_BYTES);
-            tma_load_2d_cg2(sA + stage * Cfg::A_BYTES, &tma_a, &full_bar[stage], kb * BK, m_blk * BM);
-            tma_load_2d_cg2(sB + stage * B_BYTES, &tma_b, &full_bar[stage], kb * BK, n_blk * BN + (int)cta_rank * B_ROWS);
-          } else {
-            mbar_expect_tx(&full_bar[stage], STAGE_BYTES);
-            tma_load_2d(sA + stage * Cfg::A_BYTES, &tma_a, &full_bar[stage], kb * BK, m_blk * BM);
-            tma_load_2d(sB + stage * B_BYTES, &tma_b, &full_bar[stage], kb * BK, n_blk * BN);
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+        tma_load_2d(sA + stage * Cfg::A_BYTES, &tma_a, &full_bar[stage], kb * BK, m_blk * BM);
+        tma_load_2d(sB + stage * Cfg::B_BYTES, &tma_b, &full_bar[stage], kb * BK, n_blk * BN);
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // ===================================== MMA issuer =======================================
-    if (lane == 0 && cta_rank == 0) {                       // pair mode: only the leader CTA issues MMAs
-      constexpr uint32_t idesc = make_idesc_bf16(CG2 ? 2 * BM : BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      for (int tile = worker; tile < num_tiles; tile += num_workers) {
-        mbar_wait(&tmem_empty[as], aphase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * BN;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint64_t da = make_smem_desc_sw128(base_u32 + stage * Cfg::A_BYTES, 16, 1024);
-          const uint64_t db = make_smem_desc_sw128(base_u32 + STAGES * Cfg::A_BYTES + stage * B_BYTES, 16, 1024);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            // advance 16 K-elements = 32 bytes inside the 128B swizzle atom: +2 in the (addr >> 4) field
-            if constexpr (CG2) tc_mma_bf16_cg2(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);
-            else tc_mma_bf16(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);
-          }
-          if constexpr (CG2) {
-            tc_commit_cg2(&empty_bar[stage]);                     // frees the stage in BOTH CTAs
-            if (kb == num_kb - 1) tc_commit_cg2(&tmem_full[as]);   // both CTAs' epilogues may read their half
-          } else {
-            tc_commit(&empty_bar[stage]);                    // frees this smem stage when the MMAs retire
-            if (kb == num_kb - 1) tc_commit(&tmem_full[as]);  // accumulator complete -> epilogue
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        if (++as == 2) { as = 0; aphase ^= 1; }
-      }
-    }
-  } else {
-    // ===================================== epilogue =========================================
-    const int quad = warp & 3;  // TMEM lane quadrant this warp may access
-    const int r_in_tile = quad * 32 + lane;
-    int as = 0;
-    uint32_t aphase = 0;
-    uint32_t res_ph = 0;        // TEPI: parity bits of this warp's two residual-box barriers
-    pdl_wait();                 // residual rows / row statistics of the previous kernel are read below
-    for (int tile = worker; tile < num_tiles; tile += num_workers) {
-      const int m_step = tile / p.num_n_tiles, n_blk = tile % p.num_n_tiles;
-      const int m_blk = CG2 ? 2 * m_step + (int)cta_rank : m_step;
-      const int row = m_blk * BM + r_in_tile;
-      const bool row_ok = row < p.M;
-
-      // per-column vectors of this tile -> smem once (instead of per-element global loads in every thread)
-      constexpr bool kHasVec = (EPI == EPI_BIAS || EPI == EPI_BIAS_RES_STATS || EPI == EPI_LN_BIAS || EPI == EPI_LN_BIAS_GELU);
-      float* sbias = svec + as * 2 * BN;
-      float* scol = sbias + BN;
-      if constexpr (kHasVec) {
-        const int e = threadIdx.x - 64;
-        for (int i = e; i < BN; i += 128) {
-          const int n = n_blk * BN + i;
-          sbias[i] = (p.bias != nullptr && n < p.N) ? __ldg(p.bias + n) : 0.f;
-          if constexpr (EPI == EPI_LN_BIAS || EPI == EPI_LN_BIAS_GELU) scol[i] = (n < p.N) ? __ldg(p.colsum + n) : 0.f;
-        }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-      }
-      // residual rows do not depend on the MMA: issue every load of the tile before waiting for the accumulator
-      // (TEPI: one lane starts the TMA loads of the first two 32 x 64 residual boxes of this warp's rows instead)
-      constexpr int STG_CPS = (EPI == EPI_RMS_SWIGLU) ? 4 : 2;            // 32-column accumulator chunks per 64-column output box
-      constexpr int STG_NSLAB = BN / 32 / STG_CPS;
-      uint8_t* stg = smem + STAGES * STAGE_BYTES + (warp - 2) * 3 * STG_BOX;
-      uint64_t* res_full = res_full_all + (warp - 2) * 2;
-      const int stg_row0 = m_blk * BM + quad * 32;
-      const int stg_col0 = (EPI == EPI_RMS_SWIGLU) ? (n_blk * BN) >> 1 : n_blk * BN;
-      if constexpr (TEPI && EPI == EPI_BIAS_RES_STATS) {
-        if (lane == 0) {
-#pragma unroll
-          for (int sl = 0; sl < 2 && sl < STG_NSLAB; ++sl) {
-            mbar_expect_tx(&res_full[sl], STG_BOX);
-            tma_load_2d(stg + sl * STG_BOX, &tma_r, &res_full[sl], stg_col0 + sl * 64, stg_row0);
-          }
-        }
-      }
-      uint4 resv[(EPI == EPI_BIAS_RES_STATS && !TEPI) ? BN / 8 : 1];
-      if constexpr (EPI == EPI_BIAS_RES_STATS && !TEPI) {
-        const uint4* rp = reinterpret_cast<const uint4*>(p.residual + (size_t)row * p.ldr + n_blk * BN);
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j)
-          resv[j] = (row_ok && n_blk * BN + j * 8 < p.N) ? __ldg(rp + j) : make_uint4(0, 0, 0, 0);
-      }
-
-      float mean = 0.f, rstd = 1.f;
-      if constexpr (EPI == EPI_LN_BIAS || EPI == EPI_LN_BIAS_GELU || EPI == EPI_RMS_QKV_ROPE || EPI == EPI_RMS_SWIGLU ||
-                    EPI == EPI_RMS_F32) {
-        if (row_ok) {
-          float s = 0.f, ss = 0.f;
-          const float2* st = p.stats_in + (size_t)row * p.stats_in_nt;
-          for (int i = 0; i < p.stats_in_nt; ++i) {
-            const float2 v = st[i];
-            s += v.x;
-            ss += v.y;
-          }
-          if constexpr (EPI == EPI_LN_BIAS || EPI == EPI_LN_BIAS_GELU) {
-            mean = s * p.inv_dim;
-            const float var = fmaxf(ss * p.inv_dim - mean * mean, 0.f);
-            rstd = rsqrtf(var + p.eps);
-          } else {
-            rstd = rsqrtf(ss * p.inv_dim + p.eps);
-          }
-        }
-      }
-      int b_idx = 0, pos = 0;
-      if constexpr (EPI == EPI_RMS_QKV_ROPE) {
-        if (row_ok) {
-          b_idx = row / p.S;
-          pos = p.past + (row % p.S);
-        }
-      }
-
-      __syncwarp();
-      mbar_wait(&tmem_full[as], aphase);
-      tc_fence_after();
-      float st_sum = 0.f, st_sq = 0.f;
-      long long peer_row = 0;
-      if constexpr (EPI == EPI_BIAS_RES_STATS) {
-        if (p.n_peers > 0) {
-          const int f = row / p.peer_tokens;
-          peer_row = (p.peer_frame_off + (long long)f * p.peer_frame_stride) * p.peer_tokens + (row - f * p.peer_tokens);
-        }
-      }
-      if constexpr (TEPI) {
-        // ---- output through shared memory + TMA tensor stores; residual through TMA loads (see the header) ----
-        constexpr bool kRes = (EPI == EPI_BIAS_RES_STATS);
-        const uint32_t t_acc = tmem_base + (uint32_t(quad * 32) << 16) + as * BN;
-        uint32_t rbuf[2][32];
-        __syncwarp();
-        tmem_ld_32x32(t_acc, rbuf[0]);
-#pragma unroll
-        for (int sl = 0; sl < STG_NSLAB; ++sl) {
-          uint4 rs[kRes ? 8 : 1];
-          if constexpr (kRes) {
-            mbar_wait(&res_full[sl & 1], (res_ph >> (sl & 1)) & 1u);
-            res_ph ^= 1u << (sl & 1);
-            const uint8_t* rrow = stg + (sl & 1) * STG_BOX + lane * 128;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) rs[j] = *reinterpret_cast<const uint4*>(rrow + ((j ^ (lane & 7)) << 4));
-            __syncwarp();                                   // every lane has read the box: it may be refilled
-            if (lane == 0 && sl + 2 < STG_NSLAB) {
-              mbar_expect_tx(&res_full[sl & 1], STG_BOX);
-              tma_load_2d(stg + (sl & 1) * STG_BOX, &tma_r, &res_full[sl & 1], stg_col0 + (sl + 2) * 64, stg_row0);
-            }
-          }
-          uint4 o4[8];
-#pragma unroll
-          for (int cc = 0; cc < STG_CPS; ++cc) {
-            const int c = sl * STG_CPS + cc;
-            tmem_ld_wait();
-            __syncwarp();
-            if (c + 1 < BN / 32) tmem_ld_32x32(t_acc + (c + 1) * 32, rbuf[(c + 1) & 1]);
-            const int n0 = n_blk * BN + c * 32;
-            float v[32];
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(rbuf[c & 1][i]);
-            if constexpr (EPI == EPI_BIAS || EPI == EPI_BIAS_RES_STATS) {
-              const float4* b4 = reinterpret_cast<const float4*>(sbias + c * 32);
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const float4 bb = b4[j];
-                v[4 * j] += bb.x; v[4 * j + 1] += bb.y; v[4 * j + 2] += bb.z; v[4 * j + 3] += bb.w;
-              }
-            }
-            if constexpr (EPI == EPI_LN_BIAS || EPI == EPI_LN_BIAS_GELU) {
-              const float4* b4 = reinterpret_cast<const float4*>(sbias + c * 32);
-              const float4* c4 = reinterpret_cast<const float4*>(scol + c * 32);
-              const float nm = -mean * rstd;
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const float4 bb = b4[j], cc4 = c4[j];
-                const float bq[4] = {bb.x, bb.y, bb.z, bb.w}, cq[4] = {cc4.x, cc4.y, cc4.z, cc4.w};
-#pragma unroll
-                for (int t4 = 0; t4 < 4; ++t4) {
-                  float t = fmaf(rstd, v[4 * j + t4], fmaf(nm, cq[t4], bq[t4]));   // rstd*(acc - mean*colsum) + bias
-                  if constexpr (EPI == EPI_LN_BIAS_GELU) t = quick_gelu_f(t);
-                  v[4 * j + t4] = t;
-                }
-              }
-            }
-            if constexpr (EPI == EPI_RMS_SWIGLU) {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) v[i] *= rstd;
-              uint32_t ow[8];
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                const float a = silu_f(v[4 * j]) * v[4 * j + 1];
-                const float b = silu_f(v[4 * j + 2]) * v[4 * j + 3];
-                ow[j] = pack_bf16x2(a, b);
-              }
-              o4[cc * 2] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
-              o4[cc * 2 + 1] = make_uint4(ow[4], ow[5], ow[6], ow[7]);
-            } else if constexpr (kRes) {
-              // residual add, bf16 rounding, partial row statistics of the ROUNDED values
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const uint4 rr = rs[cc * 4 + j];
-                const uint32_t rw[4] = {rr.x, rr.y, rr.z, rr.w};
-                uint32_t ow[4];
-#pragma unroll
-                for (int t = 0; t < 4; ++t) {
-                  const float a = v[j * 8 + t * 2] + bf16_lo(rw[t]);
-                  const float b = v[j * 8 + t * 2 + 1] + bf16_hi(rw[t]);
-                  ow[t] = pack_bf16x2(a, b);
-                  const float ar = bf16_lo(ow[t]), br = bf16_hi(ow[t]);
-                  st_sum += ar + br;
-                  st_sq += ar * ar + br * br;
-                }
-                o4[cc * 4 + j] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
-              }
-              if (p.n_peers > 0 && row_ok && n0 < p.N) {   // compute + collective in one kernel: the tile is pushed to every rank as it retires
-                for (int q = 0; q < p.n_peers; ++q) {
-                  uint4* pp = reinterpret_cast<uint4*>(p.peer_out[q] + (size_t)peer_row * p.ldo + n0);
-#pragma unroll
-                  for (int j = 0; j < 4; ++j) pp[j] = o4[cc * 4 + j];
-                }
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 4; ++j)
-                o4[cc * 4 + j] = make_uint4(pack_bf16x2(v[8 * j], v[8 * j + 1]), pack_bf16x2(v[8 * j + 2], v[8 * j + 3]),
-                                            pack_bf16x2(v[8 * j + 4], v[8 * j + 5]), pack_bf16x2(v[8 * j + 6], v[8 * j + 7]));
-            }
-          }
-          // the 32 x 64 box: row = lane, 16-byte chunk j at (j ^ (lane & 7)) -- the 128-byte swizzle the tensor map expects, and
-          // conflict-free for the warp's 16-byte stores.  Residual mode: ONE output box (boxes 0, 1 hold the residual ping-pong);
-          // otherwise two, alternating.
-          uint8_t* so = stg + (kRes ? 2 : (sl & 1)) * STG_BOX;
-          if (lane == 0) {                                    // the earlier store from this box has finished reading it
-            if constexpr (kRes) bulk_wait_group_read<0>();
-            else bulk_wait_group_read<1>();
-          }
-          __syncwarp();
-#pragma unroll
-          for (int j = 0; j < 8; ++j) *reinterpret_cast<uint4*>(so + lane * 128 + ((j ^ (lane & 7)) << 4)) = o4[j];
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) {
-            tma_store_2d(&tma_o, so, stg_col0 + sl * 64, stg_row0);
-            bulk_commit_group();
-          }
-        }
-      } else {
-      // one 32-column chunk: epilogue math + store
-      auto process_chunk = [&](const uint32_t (&r)[32], const int c) {
-        const int n0 = n_blk * BN + c * 32;
-        if (row_ok && n0 < p.N) {
-        float v[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-
-        if constexpr (EPI == EPI_BIAS || EPI == EPI_BIAS_RES_STATS) {
-          const float4* b4 = reinterpret_cast<const float4*>(sbias + c * 32);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 bb = b4[j];
-            v[4 * j] += bb.x; v[4 * j + 1] += bb.y; v[4 * j + 2] += bb.z; v[4 * j + 3] += bb.w;
-          }
-        }
-        if constexpr (EPI == EPI_LN_BIAS || EPI == EPI_LN_BIAS_GELU) {
-          const float4* b4 = reinterpret_cast<const float4*>(sbias + c * 32);
-          const float4* c4 = reinterpret_cast<const float4*>(scol + c * 32);
-          const float nm = -mean * rstd;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 bb = b4[j], cc = c4[j];
-            const float bq[4] = {bb.x, bb.y, bb.z, bb.w}, cq[4] = {cc.x, cc.y, cc.z, cc.w};
-#pragma unroll
-            for (int t4 = 0; t4 < 4; ++t4) {
-              float t = fmaf(rstd, v[4 * j + t4], fmaf(nm, cq[t4], bq[t4]));   // rstd*(acc - mean*colsum) + bias
-              if constexpr (EPI == EPI_LN_BIAS_GELU) t = quick_gelu_f(t);
-              v[4 * j + t4] = t;
-            }
-          }
-        }
-        if constexpr (EPI == EPI_RMS_QKV_ROPE || EPI == EPI_RMS_SWIGLU || EPI == EPI_RMS_F32) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] *= rstd;
-        }
-
-        if constexpr (EPI == EPI_BIAS_RES_STATS) {
-          // residual add, bf16 rounding, partial row statistics of the ROUNDED values
-          uint4 o[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const uint4 rr = resv[c * 4 + j];
-            const uint32_t rw[4] = {rr.x, rr.y, rr.z, rr.w};
-            uint32_t ow[4];
-#pragma unroll
-            for (int t = 0; t < 4; ++t) {
-              const float a = v[j * 8 + t * 2] + bf16_lo(rw[t]);
-              const float b = v[j * 8 + t * 2 + 1] + bf16_hi(rw[t]);
-              ow[t] = pack_bf16x2(a, b);
-              const float ar = bf16_lo(ow[t]), br = bf16_hi(ow[t]);
-              st_sum += ar + br;
-              st_sq += ar * ar + br * br;
-            }
-            o[j] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
-          }
-          uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + (size_t)row * p.ldo + n0);
-#pragma unroll
-          for (int j = 0; j < 4; ++j) op[j] = o[j];
-          if (p.n_peers > 0) {          // compute + collective in one kernel: the tile is pushed to every rank as it retires
-            for (int q = 0; q < p.n_peers; ++q) {
-              uint4* pp = reinterpret_cast<uint4*>(p.peer_out[q] + (size_t)peer_row * p.ldo + n0);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) pp[j] = o[j];
-            }
-          }
-        } else if constexpr (EPI == EPI_RMS_SWIGLU) {
-          uint32_t ow[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float a = silu_f(v[4 * j]) * v[4 * j + 1];
-            const float b = silu_f(v[4 * j + 2]) * v[4 * j + 3];
-            ow[j] = pack_bf16x2(a, b);
-          }
-          uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + (size_t)row * p.ldo + (n0 >> 1));
-          op[0] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
-          op[1] = make_uint4(ow[4], ow[5], ow[6], ow[7]);
-        } else if constexpr (EPI == EPI_RMS_F32) {
-          float* op = reinterpret_cast<float*>(p.out) + (size_t)row * p.ldo + n0;
-          if (n0 + 32 <= p.N && (p.ldo & 3) == 0) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              reinterpret_cast<float4*>(op)[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (n0 + i < p.N) op[i] = v[i];
-          }
-        } else if constexpr (EPI == EPI_RMS_QKV_ROPE) {
-          const int which = n0 / p.H;            // 0 q, 1 k, 2 v (uniform over the chunk: H % 32 == 0)
-          const int nh = n0 - which * p.H;
-          const int head = nh >> 7, cidx = nh & 127;
-          if (which < 2) {
-            // interleaved layout: columns (2j, 2j+1) hold original dims (j, j+64) of the head
-            const float2* cs = p.rope + (size_t)pos * 64 + (cidx >> 1);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const float2 c_s = __ldg(cs + j);
-              const float x0 = v[2 * j], x1 = v[2 * j + 1];
-              v[2 * j] = x0 * c_s.x - x1 * c_s.y;
-              v[2 * j + 1] = x1 * c_s.x + x0 * c_s.y;
-            }
-          }
-          __nv_bfloat16* dst;
-          if (which == 0) {
-            dst = reinterpret_cast<__nv_bfloat16*>(p.out) + (size_t)row * p.ldo + nh;
-          } else {
-            __nv_bfloat16* cache = (which == 1) ? p.kcache : p.vcache;
-            dst = cache + (((size_t)b_idx * p.nH + head) * p.Smax + pos) * 128 + cidx;
-          }
-          uint4* op = reinterpret_cast<uint4*>(dst);
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            op[j] = make_uint4(pack_bf16x2(v[8 * j], v[8 * j + 1]), pack_bf16x2(v[8 * j + 2], v[8 * j + 3]),
-                               pack_bf16x2(v[8 * j + 4], v[8 * j + 5]), pack_bf16x2(v[8 * j + 6], v[8 * j + 7]));
-        } else {
-          // EPI_BIAS / EPI_LN_BIAS / EPI_LN_BIAS_GELU -> bf16 rows
-          __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.out) + (size_t)row * p.ldo + n0;
-          if (n0 + 32 <= p.N && (p.ldo & 7) == 0) {
-            uint4* op = reinterpret_cast<uint4*>(dst);
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              op[j] = make_uint4(pack_bf16x2(v[8 * j], v[8 * j + 1]), pack_bf16x2(v[8 * j + 2], v[8 * j + 3]),
-                                 pack_bf16x2(v[8 * j + 4], v[8 * j + 5]), pack_bf16x2(v[8 * j + 6], v[8 * j + 7]));
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (n0 + i < p.N) dst[i] = __float2bfloat16_rn(v[i]);
-          }
-        }
-        }  // row_ok && n0 < N
-      };
-      // TMEM loads are asynchronous until tcgen05.wait::ld: keep the next chunk in flight while this one is processed
-      // (two register buffers) -- with K = 1024 the 8 serialised TMEM round trips of a tile were longer than its main loop
-      const uint32_t t_acc = tmem_base + (uint32_t(quad * 32) << 16) + as * BN;
-      uint32_t ra[32], rb[32];
-      __syncwarp();
-      tmem_ld_32x32(t_acc, ra);
-      constexpr int kChunkUnroll = (EPI == EPI_BIAS_RES_STATS) ? BN / 64 : 1;   // full unroll keeps resv[] in registers
-#pragma unroll kChunkUnroll
-      for (int c = 0; c < BN / 32; c += 2) {
-        tmem_ld_wait();
-        __syncwarp();
-        tmem_ld_32x32(t_acc + (c + 1) * 32, rb);
-        process_chunk(ra, c);
-        tmem_ld_wait();
-        __syncwarp();
-        if (c + 2 < BN / 32) tmem_ld_32x32(t_acc + (c + 2) * 32, ra);
-        process_chunk(rb, c + 1);
-      }
-      }
-      __syncwarp();
-      // all TMEM reads of this accumulator stage are complete -> hand it back to the MMA warp
-      tc_fence_before();
-      if constexpr (CG2) {
-        if (cta_rank == 0) mbar_arrive(&tmem_empty[as]);
-        else mbar_arrive_remote(&tmem_empty[as], 0);          // the leader's MMA thread waits for both halves
-      } else {
-        mbar_arrive(&tmem_empty[as]);
-      }
-      if constexpr (EPI == EPI_BIAS_RES_STATS) {
-        if (row_ok && p.stats_out != nullptr)
-          p.stats_out[(size_t)row * p.num_n_tiles + n_blk] = make_float2(st_sum, st_sq);
-      }
-      if (++as == 2) { as = 0; aphase ^= 1; }
-    }
-    if constexpr (TEPI) {
-      if (lane == 0) bulk_wait_group_all();    // the staging boxes stay valid (and the stores complete) before the CTA retires
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (CG2) cluster_sync_all();     // neither CTA may exit (or free TMEM) while the peer can still touch it
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (CG2) tmem_dealloc_cg2(tmem_base, Cfg::TMEM_COLS);
-    else tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+  // ===================================== consumers =========================================
+  const int ct = threadIdx.x - 128;                    // 0..255 over both consumer warpgroups
+  const int t = threadIdx.x & 127;                     // thread within this warpgroup
+  const int row0 = (wg - 1) * 64;                      // first tile row of this warpgroup
+  constexpr int NB = BN / 128;                         // m64n128 accumulators per thread
+  float acc[NB][64];
+#pragma unroll
+  for (int nb = 0; nb < NB; ++nb)
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[nb][i] = 0.f;
+  {
+    int stage = 0, prev = -1;
+    uint32_t phase = 0;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint64_t da = make_smem_desc_sw128(base_u32 + stage * Cfg::A_BYTES + row0 * 128, 16, 1024);
+      const uint64_t db = make_smem_desc_sw128(base_u32 + STAGES * Cfg::A_BYTES + stage * Cfg::B_BYTES, 16, 1024);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k)
+#pragma unroll
+        for (int nb = 0; nb < NB; ++nb)    // 128 rows of B = 16 KB further on: +1024 in the 16-byte address field
+          wgmma_ss_n128(acc[nb], da + 2 * k, db + 2 * k + nb * 1024, (kb | k) != 0);
+      wgmma_commit();
+      wgmma_wait<1>();                      // the group of the previous stage has retired: hand that stage back
+      if (prev >= 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int nb = 0; nb < NB; ++nb) wgmma_fence_regs(acc[nb]);
+  }
+
+  pdl_wait();                                          // residual rows / row statistics of the previous kernel are read below
+  // per-column vectors of this tile -> smem once (instead of per-element global loads in every thread)
+  constexpr bool kHasVec = (EPI == EPI_BIAS || EPI == EPI_BIAS_RES_STATS || EPI == EPI_LN_BIAS || EPI == EPI_LN_BIAS_GELU);
+  if constexpr (kHasVec) {
+    for (int i = ct; i < BN; i += 256) {
+      const int n = n_blk * BN + i;
+      sbias[i] = (p.bias != nullptr && n < p.N) ? __ldg(p.bias + n) : 0.f;
+      if constexpr (EPI == EPI_LN_BIAS || EPI == EPI_LN_BIAS_GELU) scol[i] = (n < p.N) ? __ldg(p.colsum + n) : 0.f;
+    }
+  }
+  // every consumer has finished reading the ring (both warpgroups' wgmma retired): it becomes the fp32 staging tile
+  asm volatile("bar.sync 1, 256;" ::: "memory");
+  float* stg = reinterpret_cast<float*>(smem);
+  {
+    const int w = t >> 5, l = t & 31;
+    const int r = row0 + w * 16 + (l >> 2), c0 = (l & 3) * 2;
+#pragma unroll
+    for (int nb = 0; nb < NB; ++nb)
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int col = nb * 128 + j * 8 + c0;
+        *reinterpret_cast<float2*>(stg + (size_t)r * Cfg::ACC_LD + col) = make_float2(acc[nb][4 * j], acc[nb][4 * j + 1]);
+        *reinterpret_cast<float2*>(stg + (size_t)(r + 8) * Cfg::ACC_LD + col) = make_float2(acc[nb][4 * j + 2], acc[nb][4 * j + 3]);
+      }
+  }
+  asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // this warpgroup's 64 rows are staged
+
+  // ===================================== epilogue =========================================
+  // two threads per row (adjacent lanes): half hf owns the 32-column chunks [hf * BN / 64, (hf + 1) * BN / 64)
+  const int r_in_tile = row0 + (t >> 1);
+  const int hf = t & 1;
+  const int row = m_blk * BM + r_in_tile;
+  const bool row_ok = row < p.M;
+
+  float mean = 0.f, rstd = 1.f;
+  if constexpr (EPI == EPI_LN_BIAS || EPI == EPI_LN_BIAS_GELU || EPI == EPI_RMS_QKV_ROPE || EPI == EPI_RMS_SWIGLU ||
+                EPI == EPI_RMS_F32) {
+    if (row_ok) {
+      float s = 0.f, ss = 0.f;
+      const float2* st = p.stats_in + (size_t)row * p.stats_in_nt;
+      for (int i = 0; i < p.stats_in_nt; ++i) {
+        const float2 v = st[i];
+        s += v.x;
+        ss += v.y;
+      }
+      if constexpr (EPI == EPI_LN_BIAS || EPI == EPI_LN_BIAS_GELU) {
+        mean = s * p.inv_dim;
+        const float var = fmaxf(ss * p.inv_dim - mean * mean, 0.f);
+        rstd = rsqrtf(var + p.eps);
+      } else {
+        rstd = rsqrtf(ss * p.inv_dim + p.eps);
+      }
+    }
+  }
+  int b_idx = 0, pos = 0;
+  if constexpr (EPI == EPI_RMS_QKV_ROPE) {
+    if (row_ok) {
+      b_idx = row / p.S;
+      pos = p.past + (row % p.S);
+    }
+  }
+  float st_sum = 0.f, st_sq = 0.f;
+  long long peer_row = 0;
+  if constexpr (EPI == EPI_BIAS_RES_STATS) {
+    if (p.n_peers > 0) {
+      const int f = row / p.peer_tokens;
+      peer_row = (p.peer_frame_off + (long long)f * p.peer_frame_stride) * p.peer_tokens + (row - f * p.peer_tokens);
+    }
+  }
+  const float* srow = stg + (size_t)r_in_tile * Cfg::ACC_LD;
+  auto process_chunk = [&](const int c) {
+    const int n0 = n_blk * BN + c * 32;
+    if (row_ok && n0 < p.N) {
+    float v[32];
+#pragma unroll
+    for (int i = 0; i < 32; i += 4) {
+      const float4 a4 = *reinterpret_cast<const float4*>(srow + c * 32 + i);
+      v[i] = a4.x; v[i + 1] = a4.y; v[i + 2] = a4.z; v[i + 3] = a4.w;
+    }
+
+    if constexpr (EPI == EPI_BIAS || EPI == EPI_BIAS_RES_STATS) {
+      const float4* b4 = reinterpret_cast<const float4*>(sbias + c * 32);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float4 bb = b4[j];
+        v[4 * j] += bb.x; v[4 * j + 1] += bb.y; v[4 * j + 2] += bb.z; v[4 * j + 3] += bb.w;
+      }
+    }
+    if constexpr (EPI == EPI_LN_BIAS || EPI == EPI_LN_BIAS_GELU) {
+      const float4* b4 = reinterpret_cast<const float4*>(sbias + c * 32);
+      const float4* c4 = reinterpret_cast<const float4*>(scol + c * 32);
+      const float nm = -mean * rstd;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float4 bb = b4[j], cc = c4[j];
+        const float bq[4] = {bb.x, bb.y, bb.z, bb.w}, cq[4] = {cc.x, cc.y, cc.z, cc.w};
+#pragma unroll
+        for (int t4 = 0; t4 < 4; ++t4) {
+          float t = fmaf(rstd, v[4 * j + t4], fmaf(nm, cq[t4], bq[t4]));   // rstd*(acc - mean*colsum) + bias
+          if constexpr (EPI == EPI_LN_BIAS_GELU) t = quick_gelu_f(t);
+          v[4 * j + t4] = t;
+        }
+      }
+    }
+    if constexpr (EPI == EPI_RMS_QKV_ROPE || EPI == EPI_RMS_SWIGLU || EPI == EPI_RMS_F32) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) v[i] *= rstd;
+    }
+
+    if constexpr (EPI == EPI_BIAS_RES_STATS) {
+      // residual add, bf16 rounding, partial row statistics of the ROUNDED values
+      uint4 o[4];
+      const uint4* rp = reinterpret_cast<const uint4*>(p.residual + (size_t)row * p.ldr + n0);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const uint4 rr = __ldg(rp + j);
+        const uint32_t rw[4] = {rr.x, rr.y, rr.z, rr.w};
+        uint32_t ow[4];
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+          const float a = v[j * 8 + t * 2] + bf16_lo(rw[t]);
+          const float b = v[j * 8 + t * 2 + 1] + bf16_hi(rw[t]);
+          ow[t] = pack_bf16x2(a, b);
+          const float ar = bf16_lo(ow[t]), br = bf16_hi(ow[t]);
+          st_sum += ar + br;
+          st_sq += ar * ar + br * br;
+        }
+        o[j] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
+      }
+      uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + (size_t)row * p.ldo + n0);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) op[j] = o[j];
+      if (p.n_peers > 0) {          // compute + collective in one kernel: the tile is pushed to every rank as it retires
+        for (int q = 0; q < p.n_peers; ++q) {
+          uint4* pp = reinterpret_cast<uint4*>(p.peer_out[q] + (size_t)peer_row * p.ldo + n0);
+#pragma unroll
+          for (int j = 0; j < 4; ++j) pp[j] = o[j];
+        }
+      }
+    } else if constexpr (EPI == EPI_RMS_SWIGLU) {
+      uint32_t ow[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float a = silu_f(v[4 * j]) * v[4 * j + 1];
+        const float b = silu_f(v[4 * j + 2]) * v[4 * j + 3];
+        ow[j] = pack_bf16x2(a, b);
+      }
+      uint4* op = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + (size_t)row * p.ldo + (n0 >> 1));
+      op[0] = make_uint4(ow[0], ow[1], ow[2], ow[3]);
+      op[1] = make_uint4(ow[4], ow[5], ow[6], ow[7]);
+    } else if constexpr (EPI == EPI_RMS_F32) {
+      float* op = reinterpret_cast<float*>(p.out) + (size_t)row * p.ldo + n0;
+      if (n0 + 32 <= p.N && (p.ldo & 3) == 0) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          reinterpret_cast<float4*>(op)[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+      } else {
+#pragma unroll
+        for (int i = 0; i < 32; ++i)
+          if (n0 + i < p.N) op[i] = v[i];
+      }
+    } else if constexpr (EPI == EPI_RMS_QKV_ROPE) {
+      const int which = n0 / p.H;            // 0 q, 1 k, 2 v (uniform over the chunk: H % 32 == 0)
+      const int nh = n0 - which * p.H;
+      const int head = nh >> 7, cidx = nh & 127;
+      if (which < 2) {
+        // interleaved layout: columns (2j, 2j+1) hold original dims (j, j+64) of the head
+        const float2* cs = p.rope + (size_t)pos * 64 + (cidx >> 1);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const float2 c_s = __ldg(cs + j);
+          const float x0 = v[2 * j], x1 = v[2 * j + 1];
+          v[2 * j] = x0 * c_s.x - x1 * c_s.y;
+          v[2 * j + 1] = x1 * c_s.x + x0 * c_s.y;
+        }
+      }
+      __nv_bfloat16* dst;
+      if (which == 0) {
+        dst = reinterpret_cast<__nv_bfloat16*>(p.out) + (size_t)row * p.ldo + nh;
+      } else {
+        __nv_bfloat16* cache = (which == 1) ? p.kcache : p.vcache;
+        dst = cache + (((size_t)b_idx * p.nH + head) * p.Smax + pos) * 128 + cidx;
+      }
+      uint4* op = reinterpret_cast<uint4*>(dst);
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        op[j] = make_uint4(pack_bf16x2(v[8 * j], v[8 * j + 1]), pack_bf16x2(v[8 * j + 2], v[8 * j + 3]),
+                           pack_bf16x2(v[8 * j + 4], v[8 * j + 5]), pack_bf16x2(v[8 * j + 6], v[8 * j + 7]));
+    } else {
+      // EPI_BIAS / EPI_LN_BIAS / EPI_LN_BIAS_GELU -> bf16 rows
+      __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.out) + (size_t)row * p.ldo + n0;
+      if (n0 + 32 <= p.N && (p.ldo & 7) == 0) {
+        uint4* op = reinterpret_cast<uint4*>(dst);
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          op[j] = make_uint4(pack_bf16x2(v[8 * j], v[8 * j + 1]), pack_bf16x2(v[8 * j + 2], v[8 * j + 3]),
+                             pack_bf16x2(v[8 * j + 4], v[8 * j + 5]), pack_bf16x2(v[8 * j + 6], v[8 * j + 7]));
+      } else {
+#pragma unroll
+        for (int i = 0; i < 32; ++i)
+          if (n0 + i < p.N) dst[i] = __float2bfloat16_rn(v[i]);
+      }
+    }
+    }  // row_ok && n0 < N
+  };
+  constexpr int CPT = BN / 64;                          // chunks per thread
+#pragma unroll
+  for (int cc = 0; cc < CPT; ++cc) process_chunk(hf * CPT + cc);
+  if constexpr (EPI == EPI_BIAS_RES_STATS) {
+    st_sum += __shfl_xor_sync(0xffffffffu, st_sum, 1);
+    st_sq += __shfl_xor_sync(0xffffffffu, st_sq, 1);
+    if (hf == 0 && row_ok && p.stats_out != nullptr) p.stats_out[(size_t)row * p.num_n_tiles + n_blk] = make_float2(st_sum, st_sq);
   }
 }
 

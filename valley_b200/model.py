@@ -341,7 +341,7 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
         self.config = config
         dev = torch.device(device if not isinstance(device, int) else f"cuda:{device}")
         if dev.type != "cuda":
-            raise _lib.VlyError("valley_b200 runs on a CUDA sm_100a device only; there is no CPU path")
+            raise _lib.VlyError("valley_b200 runs on a CUDA sm_90a device only; there is no CPU path")
         self.device = dev
         self.dtype = torch.bfloat16
         c = VlyConfig(config.hidden_size, config.num_hidden_layers, config.num_attention_heads, config.intermediate_size,

@@ -55,11 +55,9 @@ TINY_V3 = ShapeSpec("tiny-v3", 512, 2, 4, 1024, vocab_size=1032, vit_layers=2, p
 TINY_MAX = ShapeSpec("tiny-max", 512, 2, 4, 1024, vocab_size=1032, vit_layers=2, patch_pooling_method="max")
 SHAPE_7B_1L_V3 = ShapeSpec("shape-7b-1l-v3", 4096, 1, 32, 11008, vit_layers=2, patch_pooling_method="temporal_transformer")
 
-# intermediate_size = 7 x 512: the tcgen05 decode consumer (B = 2..4) walks down_proj as full 2560-column stages plus a 1024-column
-# tail stage; with VLY_UMMA_XC=512 as seven re-staged 512-column sub-phases
+# intermediate_size = 7 x 512: a wide down_proj K for the tensor-core decode consumer (B = 2..4)
 TINY_UMMA = ShapeSpec("tiny-umma", 512, 2, 4, 3584, vocab_size=1032, vit_layers=2)
-# intermediate_size = 59 x 64 (not a multiple of 512, like Llama-2-7B's 11008): the last 512-column MMA group of down_proj has five
-# 64-column panels outside the tensor maps, zero-filled by the TMA unit
+# intermediate_size = 59 x 64 (not a multiple of 512, like Llama-2-7B's 11008): down_proj's K does not divide into whole ring stages
 TINY_UMMA_RAGGED = ShapeSpec("tiny-umma-ragged", 512, 2, 4, 3776, vocab_size=1032, vit_layers=2)
 
 SPECS = {s.name: s for s in (VALLEY2_7B, VALLEY_13B, TINY, TINY_WIDE, SHAPE_7B_1L, SHAPE_13B_1L, TINY_V2, TINY_V3, TINY_MAX,
