@@ -163,6 +163,7 @@ struct vly_kv {
   int nsplit = 1, gemv_grid = 0;
   int stage_bytes = 0;                 // ring slot of the persistent decode kernel: max over its phases (pick_phase_geometry)
   int n_grid_syncs = 0;                // grid barriers per decode launch
+  int l2_hint = 1;                     // persistent decode kernel: weight copies carry L2::evict_first (StepParams::l2_hint)
   PhaseDesc* d_phases = nullptr;
   int n_phases = 0;
   unsigned int* grid_counter = nullptr;
@@ -1260,7 +1261,8 @@ extern "C" int vly_kv_create(vly_ctx* c, int batch, int max_seq, vly_kv** out) {
     kv->stage_bytes = (kv->stage_bytes + 127) & ~127;
     // Stages of this phase's size kept in flight: ~100 KB of bulk copies outstanding per SM saturate HBM; every byte beyond
     // that only lengthens the queues the latency-critical traffic (grid barrier, activation staging, attention) waits in --
-    // measured: 128 KB in flight made every barrier ~1 us slower at an unchanged streaming rate.  The ring may hold more slots
+    // measured: 128 KB in flight made every barrier ~1 us slower at an unchanged streaming rate.  (On the H100, 400 W, 13B at
+    // B = 4: an L2 prefetch running 64-192 KB per SM ahead of the ring made the step 0.7-1.5 ms slower.)  The ring may hold more slots
     // than are in flight: they absorb the consumers' hand-back latency.  VLY_MEGA_INFLIGHT_KB overrides.
     static const int env_if = getenv("VLY_MEGA_INFLIGHT_KB") ? atoi(getenv("VLY_MEGA_INFLIGHT_KB")) : 100;
     for (PhaseDesc& q : ph) {
@@ -1268,6 +1270,12 @@ extern "C" int vly_kv_create(vly_ctx* c, int batch, int max_seq, vly_kv** out) {
       const int sb = q.rows * (q.kc * 2 + pad);
       q.inflight = (env_if * 1024 + sb / 2) / sb;
       if (q.inflight < 2) q.inflight = 2;
+    }
+    // The weight stream's copies carry L2::evict_first (decode_mega.cuh, producer).  VLY_MEGA_L2_HINT=0 turns that off (A/B
+    // measurements); read per cache rather than once per process, so one process can time both.
+    {
+      const char* v = getenv("VLY_MEGA_L2_HINT");
+      kv->l2_hint = (v && *v) ? atoi(v) != 0 : 1;
     }
     if (getenv("VLY_MEGA_DBG")) {
       const int n_fit = (int)(ring_budget / kv->stage_bytes);
@@ -1646,6 +1654,7 @@ static int launch_decode_mega(vly_ctx* c, vly_kv* kv, cudaStream_t st) {
     p.attn_ikeys = (env_ik >= 16 && env_ik <= 256 && env_ik % 16 == 0) ? env_ik : 0;
   }
   p.sample = kv->d_sample;
+  p.l2_hint = kv->l2_hint;
   {
     static const bool want = getenv("VLY_MEGA_DBG") != nullptr;
     p.dbg = want ? kv->dbg : nullptr;

@@ -83,6 +83,18 @@ VLY_DEVINL void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, u
                "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
+// The same copy with an L2 cache-eviction policy (from createpolicy).
+VLY_DEVINL void bulk_load_1d_hint(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar, uint64_t policy) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;\n" ::"r"(
+                   smem_u32(smem_dst)),
+               "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
+               : "memory");
+}
+VLY_DEVINL uint64_t l2_policy_evict_first() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;\n" : "=l"(p));
+  return p;
+}
 // Programmatic dependent launch: wait = all memory of the prerequisite grids is visible; launch_dependents = the
 // next grid in the stream may start being scheduled (it still blocks in ITS wait until this grid has completed).
 VLY_DEVINL void pdl_wait() { asm volatile("griddepcontrol.wait;\n" ::: "memory"); }

@@ -74,8 +74,10 @@ struct StepParams {
   int n_stages;
   int stage_bytes;              // ring slot size: max over the phases of rows * (kc * 2 + row pad)
   int n_inflight;               // global cap on the stages in flight (PhaseDesc::inflight is the per-phase value; the ring may be deeper)
+  int l2_hint;                  // 1: the weight copies into the ring carry L2::evict_first; 0: no cache hint
   long long* dbg;               // optional [gridDim][32] cycle counters: [0..3] sync, stage-x, weight loop, attention totals;
-                                // [8 + 3*type + {0,1,2}] = stage-x, loop, trailing grid sync of every phase of that PhaseType
+                                // [8 + 3*type + {0,1,2}] = stage-x, loop, trailing grid sync of every phase of that PhaseType;
+                                // [26 + type] = cycles the producer waited for a free ring slot while filling that PhaseType
 };
 
 struct MegaCfg {
@@ -468,6 +470,14 @@ __global__ void __launch_bounds__(576, 1) decode_step_kernel(const StepParams p)
       // slots keep HBM busy.
       int wst = 0, issued = 0, confirmed = 0;
       uint32_t wph = 0;
+      long long* dbg_p = p.dbg != nullptr ? p.dbg + (size_t)blockIdx.x * 32 : nullptr;
+      if (dbg_p != nullptr)
+        for (int i = 26; i < 32; ++i) dbg_p[i] = 0;
+      // The weights are read once per step (25.7 GB at 13B, 500x the L2): their copies carry L2::evict_first, so the stream
+      // does not push out what the latency-bound parts of the step wait on -- the grid-barrier counter, the activation rows,
+      // the attention partials and the KV cache.
+      const bool hint = p.l2_hint != 0;
+      const uint64_t pol_stream = l2_policy_evict_first();
       for (int pi = 0; pi < p.n_phases; ++pi) {
         // by value: a reference would be re-read from global memory after every mbarrier asm ("memory" clobber), and the time the
         // producer needs to re-arm a freed slot comes straight out of the bytes in flight
@@ -478,29 +488,38 @@ __global__ void __launch_bounds__(576, 1) decode_step_kernel(const StepParams p)
         const int n_groups = (d.N + rows_u - 1) / rows_u;
         const int n_slices = (d.K + KCp - 1) / KCp;
         const int infl = min(d.inflight, p.n_inflight);
+        long long t_blocked = 0;
         for (int g = blockIdx.x; g < n_groups; g += gridDim.x) {
           const int n0 = g * rows_u;
           const int rows = min(rows_u, d.N - n0);
           for (int s = 0; s < n_slices; ++s) {
             const int kc = min(KCp, d.K - s * KCp);
+            const long long t_w = dbg_p != nullptr ? clock64() : 0;
             mbar_wait(&empty_bar[st], ph ^ 1);
             while (issued - confirmed >= infl) {          // at most `infl` copies outstanding: the oldest must have landed
               mbar_wait(&full_bar[wst], wph);
               if (++wst == p.n_stages) { wst = 0; wph ^= 1; }
               ++confirmed;
             }
+            if (dbg_p != nullptr) t_blocked += clock64() - t_w;
             ++issued;
             mbar_expect_tx(&full_bar[st], (uint32_t)rows * kc * 2);
             uint8_t* dst = ring + (size_t)st * p.stage_bytes;
             const __nv_bfloat16* src = d.W + (size_t)n0 * d.K + (size_t)s * KCp;
             if (PAD == 0 && kc == d.K) {                  // whole rows, unpadded: the unit is ONE contiguous block
-              bulk_load_1d(dst, src, (uint32_t)rows * kc * 2, &full_bar[st]);
+              if (hint) bulk_load_1d_hint(dst, src, (uint32_t)rows * kc * 2, &full_bar[st], pol_stream);
+              else bulk_load_1d(dst, src, (uint32_t)rows * kc * 2, &full_bar[st]);
+            } else if (hint) {
+              for (int r = 0; r < rows; ++r)
+                bulk_load_1d_hint(dst + r * row_stride, src + (size_t)r * d.K, (uint32_t)kc * 2, &full_bar[st], pol_stream);
             } else {
               for (int r = 0; r < rows; ++r) bulk_load_1d(dst + r * row_stride, src + (size_t)r * d.K, (uint32_t)kc * 2, &full_bar[st]);
             }
             if (++st == p.n_stages) { st = 0; ph ^= 1; }
           }
         }
+        // (the phase being filled, not the one being computed: the producer runs up to a ring ahead of the consumers)
+        if (dbg_p != nullptr) dbg_p[26 + d.type] += t_blocked;
       }
     }
     return;
@@ -520,7 +539,7 @@ __global__ void __launch_bounds__(576, 1) decode_step_kernel(const StepParams p)
   long long t_sync = 0, t_stage = 0, t_loop = 0, t_attn = 0, t0 = clock64();
   long long* dbg_o = (p.dbg != nullptr && ct == 0) ? p.dbg + (size_t)blockIdx.x * 32 : nullptr;
   if (dbg_o != nullptr)
-    for (int i = 8; i < 32; ++i) dbg_o[i] = 0;
+    for (int i = 8; i < 26; ++i) dbg_o[i] = 0;       // [26, 32) belong to the producer
   // ---- phase -1: x = embed[token] (decode input) ----
   {
     if (!is_fin) {
