@@ -147,7 +147,7 @@ int vly_embed_splice(vly_ctx* ctx, const int64_t* ids_dev, const int32_t* src_ma
 int vly_kv_create(vly_ctx* ctx, int batch, int max_seq, vly_kv** out);
 void vly_kv_destroy(vly_kv* kv);
 int vly_kv_seq_len(vly_kv* kv, int* out_len);   /* host-visible length (syncs the kv's stream state) */
-/* which kernel a decode step of this context launches ("decode_step_umma_kernel<4>", "decode_step_kernel<1>", ...): written,
+/* which kernel a decode step of this cache launches ("decode_step_kernel<1>", "per-op TMA-ring decode kernels", ...): written,
  * NUL-terminated, into name (capacity cap).  For reports (bench.py names the kernel its roofline describes); no GPU work. */
 int vly_kv_decode_kernel(vly_kv* kv, char* name, int cap);
 int vly_kv_reset(vly_kv* kv, void* stream);
@@ -210,9 +210,10 @@ int vly_generate(vly_ctx* ctx, vly_kv* kv, const int64_t* first_tokens_dev, int 
 int vly_kernel_launch_count(vly_ctx* ctx, int64_t* out);   /* kernels launched by this ctx so far */
 int vly_num_sms(vly_ctx* ctx, int* out);
 
-/* in-kernel cycle counters of the last decode step, filled only when the process runs with VLY_MEGA_DBG=1
- * (tools/bench_decode.py): copies n int64 values to host_out; returns 0, -1 (never enabled) or -2. */
-int vly_debug_mega_counters(long long* host_out, int n);
+/* in-kernel cycle counters of kv's last decode step (tools/bench_decode.py): copies n int64 values to host_out.  Only a
+ * cache created with VLY_MEGA_DBG set, at B <= 4, has them (VLY_ERR_STATE otherwise); VLY_ERR_INVALID when n exceeds the
+ * cache's 8192 values. */
+int vly_kv_debug_counters(vly_kv* kv, long long* host_out, int n);
 /* internal: lets the host-only translation units (host_splice.cpp, host_preprocess.cpp) set the thread-local error message */
 void vly_set_error_(const char* message);
 

@@ -1,6 +1,8 @@
-"""GPU: the L2 eviction hint on the persistent decode kernel's weight stream only changes how L2 holds the bytes, never what
-is computed: logits and token ids must be equal bit for bit with the hint off and on.  Each configuration runs in a subprocess of its own (the options are read
-from the environment when a KV cache is created) on the same seeded weights and prompt."""
+"""GPU: the persistent decode kernel's settings (DecodeSettings in api.cu: VLY_MEGA_*, VLY_ATTN_IKEYS) are read when a KV
+cache is created and stay with that cache.  Those tested here change only scheduling -- the L2 eviction hint on the weight
+stream, the ring depth, the bytes of copies in flight -- never what is computed: logits and token ids must be equal bit for
+bit to those of the reference configuration.  Each configuration runs in a subprocess of its own on the same seeded weights
+and prompt; one in-process test checks that a cache keeps its settings when the environment changes."""
 import os
 import subprocess
 import sys
@@ -45,12 +47,16 @@ np.savez(out_path, logits=torch.stack(logs, 1).numpy(), tokens=torch.cat(tok, 1)
 CONFIGS = {
     "all off": {"VLY_MEGA_L2_HINT": "0"},
     "defaults": {},
+    "2 stages": {"VLY_MEGA_STAGES": "2"},
+    "64 KB in flight": {"VLY_MEGA_INFLIGHT_KB": "64"},
 }
+SETTINGS = ("VLY_MEGA_STAGE_KB", "VLY_MEGA_ROWS", "VLY_MEGA_INFLIGHT_KB", "VLY_MEGA_STAGES", "VLY_MEGA_INFLIGHT", "VLY_ATTN_IKEYS",
+            "VLY_MEGA_L2_HINT", "VLY_MEGA_DBG")
 
 
 def _run(tmp_path, spec_name, B, S, name, env_over):
     env = dict(os.environ)
-    for k in ("VLY_MEGA_L2_HINT", "VLY_LIB_PATH"):
+    for k in SETTINGS + ("VLY_LIB_PATH",):
         env.pop(k, None)
     env.update(env_over)
     out = str(tmp_path / f"{spec_name}_{B}_{name.replace(' ', '_').replace('/', '')}.npz")
@@ -74,3 +80,38 @@ def test_decode_ring_options_are_bit_identical(tmp_path, spec_name, B, S):
         assert np.array_equal(got["logits"].view(np.uint32), ref["logits"].view(np.uint32)), f"{spec_name} B={B}: logits differ with {name}"
         assert np.array_equal(got["tokens"], ref["tokens"]), f"{spec_name} B={B}: token ids differ with {name}"
         assert np.array_equal(got["gen"], ref["gen"]), f"{spec_name} B={B}: generated ids differ with {name}"
+
+
+def test_decode_settings_are_fixed_per_cache(monkeypatch):
+    """One model, one process: a ring depth below 2 makes creating a cache fail; a cache created without the setting keeps
+    decoding the same tokens after the variable is set."""
+    import torch
+    from valley_b200 import synthetic as syn
+    from valley_b200._lib import check
+    from valley_b200.model import ValleyConfig, ValleyLlamaForCausalLM
+    for k in SETTINGS:
+        monkeypatch.delenv(k, raising=False)
+    spec, B, n = syn.SPECS["tiny-umma-ragged"], 2, 24
+    m = ValleyLlamaForCausalLM(ValleyConfig.from_spec(spec), 0)
+    m.load_state_dict(syn.iter_state_dict(spec, 1, device="cuda:0", vision=False))
+    m.logits_all_positions = False
+    ids = torch.randint(8, min(spec.vocab_size, 32000) - 16, (B, 40), generator=torch.Generator().manual_seed(7)).cuda()
+
+    monkeypatch.setenv("VLY_MEGA_STAGES", "1")
+    with pytest.raises(ValueError, match="weight ring"):
+        m.new_cache(B, 256)
+    monkeypatch.delenv("VLY_MEGA_STAGES")
+    cache = m.new_cache(B, 384)
+
+    def prefill_and_generate():
+        cache.reset()
+        with torch.no_grad():
+            nxt = m(input_ids=ids, past_key_values=cache).logits[:, -1].argmax(-1).contiguous()
+        gen = torch.empty(B, n, dtype=torch.int64, device="cuda")
+        check(m._lib.vly_generate_greedy(m._ctx, cache._h, nxt.data_ptr(), n, gen.data_ptr(), 0))
+        torch.cuda.synchronize()
+        return gen.cpu()
+
+    first = prefill_and_generate()
+    monkeypatch.setenv("VLY_MEGA_STAGES", "1")
+    assert torch.equal(prefill_and_generate(), first)

@@ -1,8 +1,10 @@
 """Steady-state decode timing (LLM only): python tools/bench_decode.py [--model valley2-7b] [--batch 1] [--steps 120]
 
---configs 'A=1,B=2;A=0' times several settings of the decode kernel's VLY_MEGA_* environment overrides in one process (the
-weights are loaded once): every configuration gets a KV cache of its own, created with its variables set, and the
-configurations are timed round-robin for --rounds rounds.  '' (an empty configuration) is the library's defaults."""
+--configs 'A=1,B=2;A=0' times several settings of the persistent decode kernel's overrides (VLY_MEGA_*, VLY_ATTN_IKEYS) in
+one process (the weights are loaded once).  The library reads them when a KV cache is created and the cache keeps them, so
+every configuration gets a KV cache of its own, created with its variables set, and the configurations are timed
+round-robin for --rounds rounds.  '' (an empty configuration) is the library's defaults.  With VLY_MEGA_DBG=1 each
+configuration's cycle counters are read from its own cache."""
 import argparse, os, statistics, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -63,14 +65,15 @@ def run_config(ci, cfg):
     e0.record(); run(a.steps); e1.record(); torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / a.steps
     S = cache.get_seq_length()
-    return ms, S, out[0, :6].tolist()
+    return ms, S, out[0, :6].tolist(), counters(cache)
 
 
-def counters():
+def counters(cache):
+    """the cycle counters of cache's last decode step, or None (the cache was not created with VLY_MEGA_DBG set, or B > 4)"""
     import ctypes as C
     import numpy as np
     buf = (C.c_longlong * (n_sm * 32))()
-    if m._lib.vly_debug_mega_counters(buf, n_sm * 32) != 0:
+    if m._lib.vly_kv_debug_counters(cache._h, buf, n_sm * 32) != 0:
         return None
     return np.array(buf[:]).reshape(n_sm, 32)
 
@@ -94,15 +97,12 @@ def print_counters(arr, ms_step):
 
 
 res = {i: [] for i in range(len(configs))}
-arrs = {}
 for rnd in range(a.rounds):
     for ci, cfg in enumerate(configs):
-        ms, S, toks = run_config(ci, cfg)
+        ms, S, toks, arr = run_config(ci, cfg)
         res[ci].append(ms)
-        if rnd == 0:        # the counter buffer read back is the one of the cache whose decode graph was captured last
-            arrs[ci] = counters() if os.environ.get("VLY_MEGA_DBG") else None
         if rnd == a.rounds - 1:
-            res[ci] = (res[ci], S, toks, arrs[ci])
+            res[ci] = (res[ci], S, toks, arr)
 os.environ.clear()
 os.environ.update(base_env)
 for ci, cfg in enumerate(configs):

@@ -84,7 +84,7 @@ SIGNATURES = {
     "vly_generate": (_i, [_vp, _vp, _vp, _i, _vp, _p(VlySampling), _vp, _vp]),
     "vly_kernel_launch_count": (_i, [_vp, _p(_i64)]),
     "vly_num_sms": (_i, [_vp, _p(_i)]),
-    "vly_debug_mega_counters": (_i, [_vp, _i]),
+    "vly_kv_debug_counters": (_i, [_vp, _vp, _i]),
     "vly_set_error_": (None, [C.c_char_p]),
     "vly_test_gemm": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp]),
     "vly_test_vit_attention": (_i, [_vp, _vp, _i, _vp, _vp]),

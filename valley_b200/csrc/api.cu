@@ -155,19 +155,17 @@ struct vly_kv {
   float* part_o = nullptr;
   float2* part_ml = nullptr;
   unsigned int* counters = nullptr;   // [B*nH] + 1 (argmax)
-  float* part_val = nullptr;
+  float* part_val = nullptr;          // [B, SMs]: per-CTA arg-max partials
   int* part_idx = nullptr;
   float* logits = nullptr;            // [B, V]
   long long* cur_tokens = nullptr;    // [B]
   long long* gen_tokens = nullptr;    // [B, Smax]
-  int nsplit = 1, gemv_grid = 0;
-  int stage_bytes = 0;                 // ring slot of the persistent decode kernel: max over its phases (pick_phase_geometry)
-  int n_grid_syncs = 0;                // grid barriers per decode launch
-  int l2_hint = 1;                     // persistent decode kernel: weight copies carry L2::evict_first (StepParams::l2_hint)
+  int nsplit = 1;
+  // persistent decode kernel (B <= 4): the whole launch, fixed by vly_kv_create
   PhaseDesc* d_phases = nullptr;
-  int n_phases = 0;
-  unsigned int* grid_counter = nullptr;
-  long long* dbg = nullptr;
+  StepParams mega = {};
+  size_t mega_smem = 0;
+  long long* dbg = nullptr;           // [SMs][32] cycle counters (StepParams::dbg); allocated only with VLY_MEGA_DBG
   SampleState* d_sample = nullptr;    // token selection state read by every decode step (sampling.cuh)
   bool sample_dirty = false;          // device state is not the plain-greedy default
   uint32_t* key_bits = nullptr;       // [B, Smax/32] attention_mask bits (1 = attend); all ones unless vly_kv_set_key_mask
@@ -192,21 +190,6 @@ static int sync_len(vly_kv* kv) {
   kv->len_dirty = false;
   return VLY_OK;
 }
-
-// decode implementation: 2 = one persistent cooperative kernel per step (default), 1 = per-op TMA-ring kernels + PDL,
-// 0 = per-op register-streaming kernels (generation 1).  VLY_DECODE=v1|ring|mega overrides (A/B measurements).
-static int decode_mode() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("VLY_DECODE");
-    v = 2;
-    if (e && !strcmp(e, "v1")) v = 0;
-    if (e && !strcmp(e, "ring")) v = 1;
-    if (getenv("VLY_DECODE_V1")) v = 0;
-  }
-  return v;
-}
-static bool use_decode_v1() { return decode_mode() == 0; }
 
 static inline int cdiv(long long a, long long b) { return int((a + b - 1) / b); }
 
@@ -1131,6 +1114,40 @@ static void mega_smem_layout(const vly_config& g, int bmax, size_t* x_bytes, siz
   *misc = (2 * MegaCfg::MAX_STAGES + 2 * MegaCfg::RED_SLOTS + 2) * 8 + (size_t)MegaCfg::RED_SLOTS * 16 * nv * 4 + (3 + 16) * bmax * 4 + 256;
 }
 static const size_t kMegaSmem = 226 * 1024;
+static const int kMegaDbgCounters = 1024 * 8;    // capacity of vly_kv::dbg: 32 per CTA
+
+// Overrides of the persistent decode kernel's launch plan, for tuning it on the GPU at hand (tools/bench_decode.py --configs).
+// They are read from the environment by read_decode_settings() and nowhere else, once per KV cache when vly_kv_create
+// builds the plan: a cache keeps the settings it was created with, whatever the environment says later.  Unset (0) keeps
+// the library's choice.
+struct DecodeSettings {
+  int stage_kb = 0;         // VLY_MEGA_STAGE_KB: target ring stage size in KB (pick_phase_geometry)
+  int rows = 0;             // VLY_MEGA_ROWS: weight rows per work unit (pick_phase_geometry)
+  int inflight_kb = 100;    // VLY_MEGA_INFLIGHT_KB: KB of bulk copies kept in flight per SM, per phase (PhaseDesc::inflight)
+  int stages = 0;           // VLY_MEGA_STAGES: ring depth cap (default 4); below 2 no cache can be created
+  int inflight = 0;         // VLY_MEGA_INFLIGHT: cap on the stages in flight over all phases (default: the ring depth)
+  int attn_ikeys = 0;       // VLY_ATTN_IKEYS: keys per attention work item, 16..256 in steps of 16 (default: by shape)
+  int l2_hint = 1;          // VLY_MEGA_L2_HINT=0: the weight copies carry no L2::evict_first policy
+  bool dbg = false;         // VLY_MEGA_DBG (any value): the kernel fills per-CTA cycle counters (vly_kv_debug_counters)
+};
+static DecodeSettings read_decode_settings() {
+  auto num = [](const char* name, int unset) {
+    const char* v = getenv(name);
+    return v ? atoi(v) : unset;
+  };
+  DecodeSettings s;
+  s.stage_kb = num("VLY_MEGA_STAGE_KB", 0);
+  s.rows = num("VLY_MEGA_ROWS", 0);
+  s.inflight_kb = num("VLY_MEGA_INFLIGHT_KB", 100);
+  s.stages = num("VLY_MEGA_STAGES", 0);
+  s.inflight = num("VLY_MEGA_INFLIGHT", 0);
+  const int ik = num("VLY_ATTN_IKEYS", 0);
+  s.attn_ikeys = (ik >= 16 && ik <= 256 && ik % 16 == 0) ? ik : 0;
+  const char* hint = getenv("VLY_MEGA_L2_HINT");
+  s.l2_hint = (hint && *hint) ? atoi(hint) != 0 : 1;
+  s.dbg = getenv("VLY_MEGA_DBG") != nullptr;
+  return s;
+}
 
 // Ring geometry of one weight phase of the persistent decode kernel: rows per work unit and columns per stage.  The rules:
 //   * HBM streams best with a bounded number of bytes of bulk copies outstanding per SM (~100 KB): fewer leave it idle, more
@@ -1141,16 +1158,15 @@ static const size_t kMegaSmem = 226 * 1024;
 //     (but 16-48 KB), cut so that K divides into EQUAL stages (no short tail stage);
 //   * rows: the candidate (max, max / 2) that satisfies the copy-size rule, then the one whose work units balance better over
 //     the SMs -- the phase lasts as long as its most loaded CTA: N = 5120 is 5 rounds of 8 rows (40) but 9 rounds of 4 (36).
-// VLY_MEGA_STAGE_KB / VLY_MEGA_ROWS override (A/B measurements).
-static void pick_phase_geometry(int bmax, size_t ring_budget, int N, int K, int num_sms, int* rows_out, int* kc_out) {
+// DecodeSettings::stage_kb / ::rows override.
+static void pick_phase_geometry(const DecodeSettings& s, int bmax, size_t ring_budget, int N, int K, int num_sms, int* rows_out,
+                                int* kc_out) {
   const bool tc = bmax > 1;
   const int max_rows = tc ? MegaCfg::ROWS_TC : MegaCfg::ROWS;
   const int pad = tc ? MegaCfg::PAD_TC : 0, gran = tc ? 64 : 8;
-  static const int env_kb = getenv("VLY_MEGA_STAGE_KB") ? atoi(getenv("VLY_MEGA_STAGE_KB")) : 0;
-  static const int env_rows = getenv("VLY_MEGA_ROWS") ? atoi(getenv("VLY_MEGA_ROWS")) : 0;
   // stage size: CUDA-core path 4 slots of ~41 KB (fewer, larger slots put more bytes in flight; more slots make the grid barriers
   // queue behind the extra prefetch traffic); tensor-core path 8 rows x ~2048 columns
-  size_t target = env_kb > 0 ? (size_t)env_kb * 1024 : (tc ? 33 * 1024 + 512 : 41 * 1024);
+  size_t target = s.stage_kb > 0 ? (size_t)s.stage_kb * 1024 : (tc ? 33 * 1024 + 512 : 41 * 1024);
   if (target > ring_budget / 2) target = ring_budget / 2;
   if (target < 8 * 1024) target = 8 * 1024;
   auto kc_for = [&](int rows) {
@@ -1160,7 +1176,7 @@ static void pick_phase_geometry(int bmax, size_t ring_budget, int N, int K, int 
     return kc > K ? cdiv(K, gran) * gran : kc;
   };
   int rows = max_rows;
-  if (env_rows > 0) rows = env_rows > max_rows ? max_rows : env_rows;
+  if (s.rows > 0) rows = s.rows > max_rows ? max_rows : s.rows;
   else {
     if (kc_for(rows) * 2 < 3072 && K * 2 >= 3072) rows = max_rows / 2;            // keep every bulk copy >= 3 KB
     if (rows == max_rows && !tc) {        // (tensor-core path: half-filled HMMAs cost more than the imbalance they would remove)
@@ -1171,6 +1187,101 @@ static void pick_phase_geometry(int bmax, size_t ring_budget, int N, int K, int 
   }
   *rows_out = rows;
   *kc_out = kc_for(rows);
+}
+
+// The complete launch of the persistent decode-step kernel for kv (B <= 4): phase table, ring geometry and depth, shared memory
+// and StepParams.  Everything it depends on -- shapes, weight and cache pointers, settings -- is fixed once the cache exists.
+static int plan_decode_mega(vly_ctx* c, vly_kv* kv, const DecodeSettings& s) {
+  const vly_config& g = c->cfg;
+  const int B = kv->B, H = g.hidden_size, nH = g.num_attention_heads, I = g.intermediate_size, V = g.vocab_size;
+  const int bmax = B <= 1 ? 1 : (B <= 2 ? 2 : 4);
+  const int pad = bmax > 1 ? MegaCfg::PAD_TC : 0;
+  size_t x_bytes, misc;
+  mega_smem_layout(g, bmax, &x_bytes, &misc);
+  const size_t ring_budget = kMegaSmem > x_bytes + misc ? kMegaSmem - x_bytes - misc : 0;
+  // phase table: execution order of one step
+  std::vector<PhaseDesc> ph;
+  int stage_bytes = 0;
+  auto add = [&](PhaseDesc d) {
+    d.rows = d.kc = 0;
+    if (d.type != PH_ATTN) {
+      pick_phase_geometry(s, bmax, ring_budget, d.N, d.K, c->num_sms, &d.rows, &d.kc);
+      const int sb = d.rows * (d.kc * 2 + pad);
+      if (sb > stage_bytes) stage_bytes = sb;
+    }
+    ph.push_back(d);
+  };
+  for (int l = 0; l < g.num_hidden_layers; ++l) {
+    const LlamaLayerW& w = c->layers[l];
+    PhaseDesc d = {};
+    d.layer = l; d.kcache = kv->k_layer(l); d.vcache = kv->v_layer(l);
+    d.type = PH_QKV; d.N = 3 * H; d.K = H; d.W = w.wqkv; d.x_in = kv->x; d.out = kv->q; add(d);
+    d.type = PH_ATTN; d.N = 0; d.K = 0; d.W = nullptr; d.x_in = nullptr; d.out = kv->attn; add(d);
+    d.type = PH_OPROJ; d.N = H; d.K = H; d.W = w.wo; d.x_in = kv->attn; d.out = kv->x; add(d);
+    d.type = PH_GATEUP; d.N = 2 * I; d.K = H; d.W = w.wgu; d.x_in = kv->x; d.out = kv->hb; add(d);
+    d.type = PH_DOWN; d.N = H; d.K = I; d.W = w.wdown; d.x_in = kv->hb; d.out = kv->x; add(d);
+  }
+  {
+    PhaseDesc d = {};
+    d.type = PH_LOGITS; d.N = V; d.K = H; d.W = c->lm_head; d.x_in = kv->x; d.out = nullptr; add(d);
+  }
+  stage_bytes = (stage_bytes + 127) & ~127;
+  // Stages of this phase's size kept in flight: ~100 KB of bulk copies outstanding per SM saturate HBM; every byte beyond
+  // that only lengthens the queues the latency-critical traffic (grid barrier, activation staging, attention) waits in --
+  // measured: 128 KB in flight made every barrier ~1 us slower at an unchanged streaming rate.  (On the H100, 400 W, 13B at
+  // B = 4: an L2 prefetch running 64-192 KB per SM ahead of the ring made the step 0.7-1.5 ms slower.)  The ring may hold more slots
+  // than are in flight: they absorb the consumers' hand-back latency.
+  for (PhaseDesc& q : ph) {
+    if (q.type == PH_ATTN) continue;
+    const int sb = q.rows * (q.kc * 2 + pad);
+    q.inflight = (s.inflight_kb * 1024 + sb / 2) / sb;
+    if (q.inflight < 2) q.inflight = 2;
+  }
+  // depth of the ring: what fits next to the activation block, at most 4 (deeper rings made every grid barrier slower, see
+  // pick_phase_geometry)
+  int n_stages = (int)(((long long)kMegaSmem - (long long)x_bytes - (long long)misc) / (long long)stage_bytes);
+  if (n_stages > MegaCfg::MAX_STAGES) n_stages = MegaCfg::MAX_STAGES;
+  const int cap = s.stages > 0 ? s.stages : 4;
+  if (n_stages > cap) n_stages = cap;
+  if (n_stages < 2)
+    return fail(VLY_ERR_INVALID, "vly_kv_create: activations (B=%d, K=%d) leave no room for the weight ring (%d stages, at least 2 needed)",
+                B, std::max(I, H), n_stages);
+  if (s.dbg) {
+    fprintf(stderr, "[vly] decode ring: B=%d x=%zu B, ring budget %zu B, slot %d B, %d slots fit, %d used;", B, x_bytes, ring_budget,
+            stage_bytes, (int)(ring_budget / stage_bytes), n_stages);
+    for (int i = 0; i < 5 && i < (int)ph.size(); ++i)
+      if (ph[i].type != PH_ATTN) fprintf(stderr, " type%d N=%d K=%d rows=%d kc=%d inflight=%d;", ph[i].type, ph[i].N, ph[i].K, ph[i].rows, ph[i].kc, ph[i].inflight);
+    fprintf(stderr, " logits rows=%d kc=%d\n", ph.back().rows, ph.back().kc);
+    CK(cudaMalloc((void**)&kv->dbg, kMegaDbgCounters * sizeof(long long)));
+  }
+  CK(cudaMalloc((void**)&kv->d_phases, ph.size() * sizeof(PhaseDesc)));
+  CK(cudaMemcpy(kv->d_phases, ph.data(), ph.size() * sizeof(PhaseDesc), cudaMemcpyHostToDevice));
+
+  StepParams& p = kv->mega;
+  p = {};
+  p.phases = kv->d_phases; p.n_phases = (int)ph.size();
+  p.B = B; p.H = H; p.nH = nH; p.Smax = kv->Smax; p.V = V;
+  p.Kmax = std::max(I, H);
+  p.eps = g.rms_norm_eps; p.scale_log2e = 0.08838834764831845f * 1.4426950408889634f;
+  p.rope = c->rope; p.seq_len = kv->d_len; p.step = kv->d_step; p.embed = c->embed; p.tokens_in = kv->cur_tokens;
+  p.x = kv->x; p.q = kv->q; p.attn = kv->attn;
+  p.part_o = kv->part_o; p.part_ml = kv->part_ml; p.attn_counters = kv->counters; p.nsplit = kv->nsplit;
+  p.key_bits = kv->key_bits; p.mask_words = kv->mask_words();
+  p.logits = kv->logits; p.part_val = kv->part_val; p.part_idx = kv->part_idx;
+  p.next_tokens = kv->cur_tokens; p.out_tokens = kv->gen_tokens; p.out_stride = kv->Smax;
+  p.sample = kv->d_sample;
+  p.grid_counter = kv->counters + (size_t)B * nH + 1;
+  p.grid_epoch = p.grid_counter + 1;
+  p.n_grid_syncs = p.n_phases + 1;               // one per phase + the embedding phase
+  p.attn_ikeys = s.attn_ikeys;
+  p.n_stages = n_stages;
+  p.stage_bytes = stage_bytes;
+  p.n_inflight = s.inflight > 0 ? s.inflight : n_stages;      // (PhaseDesc::inflight is the per-phase value)
+  if (p.n_inflight > n_stages) p.n_inflight = n_stages;
+  p.l2_hint = s.l2_hint;
+  p.dbg = kv->dbg;
+  kv->mega_smem = (size_t)n_stages * stage_bytes + x_bytes + misc;
+  return VLY_OK;
 }
 
 extern "C" int vly_kv_create(vly_ctx* c, int batch, int max_seq, vly_kv** out) {
@@ -1187,15 +1298,8 @@ extern "C" int vly_kv_create(vly_ctx* c, int batch, int max_seq, vly_kv** out) {
   const size_t cache_elems = (size_t)L * kv->layer_stride();
   CK(cudaMalloc((void**)&kv->cache, cache_elems * 2));
   CK(cudaMemset(kv->cache, 0, cache_elems * 2));   // padded keys must be finite: P(=0) * V(pad) must stay 0
-  // split-KV factor: enough CTAs to cover the GPU about twice
-  if (decode_mode() == 0) {
-    int ns = (2 * c->num_sms + batch * nH - 1) / (batch * nH);
-    kv->nsplit = ns < 1 ? 1 : (ns > 16 ? 16 : ns);
-  } else {
-    kv->nsplit = kv->Smax / MegaCfg::ATTN_KEYS_MIN; // capacity of the split dimension: the persistent kernel uses 16/32-key items, the
-                                                // per-op kernel fixed 64-key splits (it only touches the first Smax / 64 slots)
-  }
-  kv->gemv_grid = 2 * c->num_sms;
+  kv->nsplit = kv->Smax / MegaCfg::ATTN_KEYS_MIN;   // capacity of the split dimension: the persistent kernel uses 16/32-key items,
+                                                    // the per-op kernel fixed 64-key splits (it only touches the first Smax / 64 slots)
   CK(cudaMalloc((void**)&kv->d_len, 8));
   CK(cudaHostAlloc((void**)&kv->h_len, sizeof(int), cudaHostAllocDefault));
   CK(cudaEventCreateWithFlags(&kv->len_event, cudaEventDisableTiming));
@@ -1214,13 +1318,11 @@ extern "C" int vly_kv_create(vly_ctx* c, int batch, int max_seq, vly_kv** out) {
   CK(cudaMalloc((void**)&kv->part_ml, (size_t)batch * nH * kv->nsplit * sizeof(float2)));
   CK(cudaMalloc((void**)&kv->counters, ((size_t)batch * nH + 4) * 4));
   CK(cudaMemset(kv->counters, 0, ((size_t)batch * nH + 4) * 4));
-  kv->grid_counter = kv->counters + (size_t)batch * nH + 1;      // [+2] = launch epoch of the grid barrier
-  CK(cudaMalloc((void**)&kv->part_val, (size_t)batch * kv->gemv_grid * 4));
-  CK(cudaMalloc((void**)&kv->part_idx, (size_t)batch * kv->gemv_grid * 4));
+  CK(cudaMalloc((void**)&kv->part_val, (size_t)batch * c->num_sms * 4));   // every arg-max kernel runs at most one CTA per SM
+  CK(cudaMalloc((void**)&kv->part_idx, (size_t)batch * c->num_sms * 4));
   CK(cudaMalloc((void**)&kv->logits, (size_t)batch * V * 4));
   CK(cudaMalloc((void**)&kv->cur_tokens, (size_t)batch * 8));
   CK(cudaMalloc((void**)&kv->gen_tokens, (size_t)batch * kv->Smax * 8));
-  CK(cudaMalloc((void**)&kv->dbg, 1024 * 8 * 8));
   CK(cudaMalloc((void**)&kv->d_sample, sizeof(SampleState)));
   {
     SampleState s0 = {};
@@ -1229,65 +1331,12 @@ extern "C" int vly_kv_create(vly_ctx* c, int batch, int max_seq, vly_kv** out) {
   }
   CK(cudaMalloc((void**)&kv->key_bits, (size_t)batch * kv->mask_words() * 4));
   CK(cudaMemset(kv->key_bits, 0xff, (size_t)batch * kv->mask_words() * 4));
-  {  // phase table of the persistent decode-step kernel: execution order of one step
-    std::vector<PhaseDesc> ph;
-    const int bmax = batch <= 1 ? 1 : (batch <= 2 ? 2 : 4);
-    const int pad = bmax > 1 ? MegaCfg::PAD_TC : 0;
-    size_t x_bytes, misc;
-    mega_smem_layout(g, bmax, &x_bytes, &misc);
-    const size_t ring_budget = kMegaSmem > x_bytes + misc ? kMegaSmem - x_bytes - misc : 0;
-    kv->stage_bytes = 0;
-    auto add = [&](PhaseDesc d) {
-      d.rows = d.kc = 0;
-      if (d.type != PH_ATTN) {
-        pick_phase_geometry(bmax, ring_budget, d.N, d.K, c->num_sms, &d.rows, &d.kc);
-        const int sb = d.rows * (d.kc * 2 + pad);
-        if (sb > kv->stage_bytes) kv->stage_bytes = sb;
-      }
-      ph.push_back(d);
-    };
-    for (int l = 0; l < L; ++l) {
-      const LlamaLayerW& w = c->layers[l];
-      PhaseDesc d = {};
-      d.layer = l; d.kcache = kv->k_layer(l); d.vcache = kv->v_layer(l);
-      d.type = PH_QKV; d.N = 3 * H; d.K = H; d.W = w.wqkv; d.x_in = kv->x; d.out = kv->q; add(d);
-      d.type = PH_ATTN; d.N = 0; d.K = 0; d.W = nullptr; d.x_in = nullptr; d.out = kv->attn; add(d);
-      d.type = PH_OPROJ; d.N = H; d.K = H; d.W = w.wo; d.x_in = kv->attn; d.out = kv->x; add(d);
-      d.type = PH_GATEUP; d.N = 2 * I; d.K = H; d.W = w.wgu; d.x_in = kv->x; d.out = kv->hb; add(d);
-      d.type = PH_DOWN; d.N = H; d.K = I; d.W = w.wdown; d.x_in = kv->hb; d.out = kv->x; add(d);
+  if (batch <= 4) {
+    const int r = plan_decode_mega(c, kv, read_decode_settings());
+    if (r != VLY_OK) {
+      vly_kv_destroy(kv);
+      return r;
     }
-    PhaseDesc d = {};
-    d.type = PH_LOGITS; d.N = V; d.K = H; d.W = c->lm_head; d.x_in = kv->x; d.out = nullptr; add(d);
-    kv->stage_bytes = (kv->stage_bytes + 127) & ~127;
-    // Stages of this phase's size kept in flight: ~100 KB of bulk copies outstanding per SM saturate HBM; every byte beyond
-    // that only lengthens the queues the latency-critical traffic (grid barrier, activation staging, attention) waits in --
-    // measured: 128 KB in flight made every barrier ~1 us slower at an unchanged streaming rate.  (On the H100, 400 W, 13B at
-    // B = 4: an L2 prefetch running 64-192 KB per SM ahead of the ring made the step 0.7-1.5 ms slower.)  The ring may hold more slots
-    // than are in flight: they absorb the consumers' hand-back latency.  VLY_MEGA_INFLIGHT_KB overrides.
-    static const int env_if = getenv("VLY_MEGA_INFLIGHT_KB") ? atoi(getenv("VLY_MEGA_INFLIGHT_KB")) : 100;
-    for (PhaseDesc& q : ph) {
-      if (q.type == PH_ATTN) continue;
-      const int sb = q.rows * (q.kc * 2 + pad);
-      q.inflight = (env_if * 1024 + sb / 2) / sb;
-      if (q.inflight < 2) q.inflight = 2;
-    }
-    // The weight stream's copies carry L2::evict_first (decode_mega.cuh, producer).  VLY_MEGA_L2_HINT=0 turns that off (A/B
-    // measurements); read per cache rather than once per process, so one process can time both.
-    {
-      const char* v = getenv("VLY_MEGA_L2_HINT");
-      kv->l2_hint = (v && *v) ? atoi(v) != 0 : 1;
-    }
-    if (getenv("VLY_MEGA_DBG")) {
-      const int n_fit = (int)(ring_budget / kv->stage_bytes);
-      fprintf(stderr, "[vly] decode ring: B=%d x=%zu B, ring budget %zu B, slot %d B, %d slots fit;", batch, x_bytes, ring_budget, kv->stage_bytes, n_fit);
-      for (int i = 0; i < 5 && i < (int)ph.size(); ++i)
-        if (ph[i].type != PH_ATTN) fprintf(stderr, " type%d N=%d K=%d rows=%d kc=%d inflight=%d;", ph[i].type, ph[i].N, ph[i].K, ph[i].rows, ph[i].kc, ph[i].inflight);
-      fprintf(stderr, " logits rows=%d kc=%d\n", ph.back().rows, ph.back().kc);
-    }
-    kv->n_phases = (int)ph.size();
-    kv->n_grid_syncs = kv->n_phases + 1;
-    CK(cudaMalloc((void**)&kv->d_phases, ph.size() * sizeof(PhaseDesc)));
-    CK(cudaMemcpy(kv->d_phases, ph.data(), ph.size() * sizeof(PhaseDesc), cudaMemcpyHostToDevice));
   }
   *out = kv;
   return VLY_OK;
@@ -1296,8 +1345,8 @@ extern "C" int vly_kv_create(vly_ctx* c, int batch, int max_seq, vly_kv** out) {
 extern "C" int vly_kv_decode_kernel(vly_kv* kv, char* name, int cap) {
   if (!kv || !name || cap <= 0) return fail(VLY_ERR_INVALID, "vly_kv_decode_kernel: bad argument");
   const int bmax = kv->B <= 1 ? 1 : (kv->B <= 2 ? 2 : 4);
-  if (decode_mode() == 2 && kv->B <= 4) snprintf(name, (size_t)cap, "decode_step_kernel<%d>", bmax);
-  else snprintf(name, (size_t)cap, "%s", decode_mode() == 0 ? "per-op decode kernels (generation 1)" : "per-op TMA-ring decode kernels");
+  if (kv->B <= 4) snprintf(name, (size_t)cap, "decode_step_kernel<%d>", bmax);
+  else snprintf(name, (size_t)cap, "per-op TMA-ring decode kernels");
   return VLY_OK;
 }
 
@@ -1378,31 +1427,7 @@ extern "C" int vly_kv_export(vly_ctx* c, vly_kv* kv, int layer, int which, void*
 // ------------------------------------------------------------------------------------------------
 // decode-side launchers
 // ------------------------------------------------------------------------------------------------
-static size_t gemv_smem(int bmax, int K) { return (size_t)bmax * K * 2 + (size_t)(2 * 8 * 8 * bmax + 2 * 8 * bmax + 3 * bmax) * 4 + 64; }
-
-template <int MODE>
-static int launch_gemv(vly_ctx* c, GemvParams p, int grid, cudaStream_t st) {
-  const int bmax = p.B <= 1 ? 1 : (p.B <= 2 ? 2 : 4);
-  if (p.B > 4) return fail(VLY_ERR_INVALID, "gemv: batch %d > 4 per call (callers split the batch)", p.B);
-  if (p.ldx == 0) p.ldx = p.K;
-  const size_t smem = gemv_smem(bmax, p.K);
-  const int units = (p.N + 7) / 8;
-  if (grid > units) grid = units;
-#define VLY_GEMV_CASE(BM)                                                                                              \
-  {                                                                                                                    \
-    TRY(ensure_smem_attr(c->cfg.device, gemv_kernel<BM, MODE>, smem));                                                 \
-    gemv_kernel<BM, MODE><<<grid, 256, smem, st>>>(p);                                                                 \
-  }
-  if (bmax == 1) VLY_GEMV_CASE(1)
-  else if (bmax == 2) VLY_GEMV_CASE(2)
-  else VLY_GEMV_CASE(4)
-#undef VLY_GEMV_CASE
-  c->launches++;
-  CKL();
-  return VLY_OK;
-}
-
-// ---- generation-2 decode launchers (TMA ring + programmatic dependent launch) ----
+// ---- per-op decode launchers (TMA ring + programmatic dependent launch) ----
 template <int MODE>
 static int launch_gemv_ring(vly_ctx* c, GemvParams p, bool pdl, cudaStream_t st) {
   const int bmax = p.B <= 1 ? 1 : (p.B <= 2 ? 2 : 4);
@@ -1444,8 +1469,6 @@ static int enqueue_decode_step(vly_ctx* c, vly_kv* kv, int b0, int nb, bool bump
   decode_embed_kernel<<<nb, 256, 0, st>>>(kv->cur_tokens + b0, c->embed, x, H, V);
   c->launches++;
   CKL();
-  const size_t attn_smem = ((size_t)kv->Smax / kv->nsplit + 8) * 4;
-  if (attn_smem > 40000) TRY(ensure_smem_attr(c->cfg.device, decode_attention_kernel, attn_smem));
   for (int l = 0; l < g.num_hidden_layers; ++l) {
     const LlamaLayerW& w = c->layers[l];
     bf16* kc = kv->k_layer(l) + (size_t)b0 * nH * kv->Smax * 128;
@@ -1454,13 +1477,12 @@ static int enqueue_decode_step(vly_ctx* c, vly_kv* kv, int b0, int nb, bool bump
       GemvParams p = {};
       p.N = 3 * H; p.K = H; p.B = nb; p.W = w.wqkv; p.x = x; p.eps = g.rms_norm_eps;
       p.out = q; p.rope = c->rope; p.seq_len = kv->d_len; p.H = H; p.nH = nH; p.Smax = kv->Smax; p.kcache = kc; p.vcache = vc;
-      if (use_decode_v1()) TRY(launch_gemv<GEMV_QKV_ROPE>(c, p, kv->gemv_grid, st));
-      else TRY(launch_gemv_ring<GEMV_QKV_ROPE>(c, p, true, st));
+      TRY(launch_gemv_ring<GEMV_QKV_ROPE>(c, p, true, st));
     }
     {
       DecAttnParams p = {};
       p.B = nb; p.nH = nH; p.H = H; p.Smax = kv->Smax; p.seq_len = kv->d_len;
-      p.nsplit = use_decode_v1() ? kv->nsplit : kv->Smax / kDecSplitKeys;
+      p.nsplit = kv->Smax / kDecSplitKeys;
       p.q = q; p.kcache = kc; p.vcache = vc;
       p.part_o = kv->part_o + (size_t)b0 * nH * kv->nsplit * 128;
       p.part_ml = kv->part_ml + (size_t)b0 * nH * kv->nsplit;
@@ -1468,42 +1490,33 @@ static int enqueue_decode_step(vly_ctx* c, vly_kv* kv, int b0, int nb, bool bump
       p.out = attn;
       p.scale_log2e = 0.08838834764831845f * 1.4426950408889634f;
       p.key_bits = kv->key_bits + (size_t)b0 * kv->mask_words(); p.mask_words = kv->mask_words();
-      if (use_decode_v1()) {
-        dim3 grid(nb * nH, kv->nsplit);
-        decode_attention_kernel<<<grid, 128, attn_smem, st>>>(p);
-        CKL();
-      } else {
-        TRY(ensure_smem_attr(c->cfg.device, decode_attention_v2_kernel, 0, true));
-        dim3 grid(nb * nH, p.nsplit);
-        CK(launch_ex(decode_attention_v2_kernel, grid, dim3(128), 0, st, true, p));
-      }
+      TRY(ensure_smem_attr(c->cfg.device, decode_attention_v2_kernel, 0, true));
+      dim3 grid(nb * nH, p.nsplit);
+      CK(launch_ex(decode_attention_v2_kernel, grid, dim3(128), 0, st, true, p));
       c->launches++;
     }
     {
       GemvParams p = {};
       p.N = H; p.K = H; p.B = nb; p.W = w.wo; p.x = attn; p.out = x; p.res = x;
-      if (use_decode_v1()) TRY(launch_gemv<GEMV_RESIDUAL>(c, p, kv->gemv_grid, st));
-      else TRY(launch_gemv_ring<GEMV_RESIDUAL>(c, p, true, st));
+      TRY(launch_gemv_ring<GEMV_RESIDUAL>(c, p, true, st));
     }
     {
       GemvParams p = {};
       p.N = 2 * I; p.K = H; p.B = nb; p.W = w.wgu; p.x = x; p.eps = g.rms_norm_eps; p.out = hb;
-      if (use_decode_v1()) TRY(launch_gemv<GEMV_SWIGLU>(c, p, kv->gemv_grid, st));
-      else TRY(launch_gemv_ring<GEMV_SWIGLU>(c, p, true, st));
+      TRY(launch_gemv_ring<GEMV_SWIGLU>(c, p, true, st));
     }
     {
       GemvParams p = {};
       p.N = H; p.K = I; p.B = nb; p.W = w.wdown; p.x = hb; p.out = x; p.res = x;
-      if (use_decode_v1()) TRY(launch_gemv<GEMV_RESIDUAL>(c, p, kv->gemv_grid, st));
-      else TRY(launch_gemv_ring<GEMV_RESIDUAL>(c, p, true, st));
+      TRY(launch_gemv_ring<GEMV_RESIDUAL>(c, p, true, st));
     }
   }
   {
     GemvParams p = {};
     p.N = V; p.K = H; p.B = nb; p.W = c->lm_head; p.x = x; p.eps = g.rms_norm_eps;
     p.logits = kv->logits + (size_t)b0 * V;
-    p.part_val = kv->part_val + (size_t)b0 * kv->gemv_grid;
-    p.part_idx = kv->part_idx + (size_t)b0 * kv->gemv_grid;
+    p.part_val = kv->part_val + (size_t)b0 * c->num_sms;
+    p.part_idx = kv->part_idx + (size_t)b0 * c->num_sms;
     p.counter = kv->counters + (size_t)kv->B * nH;
     p.next_tokens = kv->cur_tokens + b0;
     p.out_tokens = kv->gen_tokens + (size_t)b0 * kv->Smax;
@@ -1511,8 +1524,7 @@ static int enqueue_decode_step(vly_ctx* c, vly_kv* kv, int b0, int nb, bool bump
     p.step = kv->d_step;
     p.seq_len_rw = kv->d_len;
     p.bump = bump ? 1 : 0;   // only the last batch group of a step advances the step / length counters
-    if (use_decode_v1()) TRY(launch_gemv<GEMV_LOGITS>(c, p, kv->gemv_grid, st));
-    else TRY(launch_gemv_ring<GEMV_LOGITS>(c, p, true, st));
+    TRY(launch_gemv_ring<GEMV_LOGITS>(c, p, true, st));
   }
   return VLY_OK;
 }
@@ -1606,14 +1618,13 @@ extern "C" int vly_llama_prefill(vly_ctx* c, vly_kv* kv, const void* inputs_embe
     p.N = V; p.K = H; p.B = nb; p.W = c->lm_head; p.x = x + ((size_t)b0 * S + (S - 1)) * H; p.ldx = (long long)S * H;
     p.eps = g.rms_norm_eps;
     p.logits = kv->logits + (size_t)b0 * V;
-    p.part_val = kv->part_val + (size_t)b0 * kv->gemv_grid;
-    p.part_idx = kv->part_idx + (size_t)b0 * kv->gemv_grid;
+    p.part_val = kv->part_val + (size_t)b0 * c->num_sms;
+    p.part_idx = kv->part_idx + (size_t)b0 * c->num_sms;
     p.counter = kv->counters + (size_t)kv->B * nH;
     p.next_tokens = kv->cur_tokens + b0;
     p.out_tokens = nullptr;
     p.step = kv->d_step; p.seq_len_rw = kv->d_len; p.bump = 0;
-    if (use_decode_v1()) TRY(launch_gemv<GEMV_LOGITS>(c, p, kv->gemv_grid, st));
-    else TRY(launch_gemv_ring<GEMV_LOGITS>(c, p, false, st));
+    TRY(launch_gemv_ring<GEMV_LOGITS>(c, p, false, st));
   }
   if (logits_mode == 1) CK(cudaMemcpyAsync(logits_dev, kv->logits, (size_t)B * V * 4, cudaMemcpyDeviceToDevice, st));
   if (next_tokens_dev) CK(cudaMemcpyAsync(next_tokens_dev, kv->cur_tokens, (size_t)B * 8, cudaMemcpyDeviceToDevice, st));
@@ -1627,63 +1638,25 @@ extern "C" int vly_llama_prefill(vly_ctx* c, vly_kv* kv, const void* inputs_embe
 // ------------------------------------------------------------------------------------------------
 // decode
 // ------------------------------------------------------------------------------------------------
-static long long* g_mega_dbg = nullptr;
-extern "C" int vly_debug_mega_counters(long long* host_out, int n) {
-  if (!g_mega_dbg) return -1;
-  return cudaMemcpy(host_out, g_mega_dbg, (size_t)n * 8, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : -2;
+extern "C" int vly_kv_debug_counters(vly_kv* kv, long long* host_out, int n) {
+  if (!kv || !host_out || n < 0) return fail(VLY_ERR_INVALID, "vly_kv_debug_counters: bad argument");
+  if (!kv->dbg)
+    return fail(VLY_ERR_STATE, "vly_kv_debug_counters: this cache has no counters (B %d; they need B <= 4 and VLY_MEGA_DBG set when it was created)", kv->B);
+  if (n > kMegaDbgCounters) return fail(VLY_ERR_INVALID, "vly_kv_debug_counters: %d values requested, the cache holds %d", n, kMegaDbgCounters);
+  CK(cudaSetDevice(kv->ctx->cfg.device));
+  CK(cudaMemcpy(host_out, kv->dbg, (size_t)n * sizeof(long long), cudaMemcpyDeviceToHost));
+  return VLY_OK;
 }
+
+// the launch was planned by vly_kv_create (plan_decode_mega)
 static int launch_decode_mega(vly_ctx* c, vly_kv* kv, cudaStream_t st) {
-  const vly_config& g = c->cfg;
-  const int B = kv->B, bmax = B <= 1 ? 1 : (B <= 2 ? 2 : 4);
-  StepParams p = {};
-  p.phases = kv->d_phases; p.n_phases = kv->n_phases;
-  p.B = B; p.H = g.hidden_size; p.nH = g.num_attention_heads; p.Smax = kv->Smax; p.V = g.vocab_size;
-  p.Kmax = g.intermediate_size > g.hidden_size ? g.intermediate_size : g.hidden_size;
-  p.eps = g.rms_norm_eps; p.scale_log2e = 0.08838834764831845f * 1.4426950408889634f;
-  p.rope = c->rope; p.seq_len = kv->d_len; p.step = kv->d_step; p.embed = c->embed; p.tokens_in = kv->cur_tokens;
-  p.x = kv->x; p.q = kv->q; p.attn = kv->attn;
-  p.part_o = kv->part_o; p.part_ml = kv->part_ml; p.attn_counters = kv->counters; p.nsplit = kv->nsplit;
-  p.key_bits = kv->key_bits; p.mask_words = kv->mask_words();
-  p.logits = kv->logits; p.part_val = kv->part_val; p.part_idx = kv->part_idx;
-  p.next_tokens = kv->cur_tokens; p.out_tokens = kv->gen_tokens; p.out_stride = kv->Smax;
-  p.grid_counter = kv->grid_counter;
-  p.grid_epoch = kv->grid_counter + 1;
-  p.n_grid_syncs = kv->n_grid_syncs;
-  {
-    static const int env_ik = getenv("VLY_ATTN_IKEYS") ? atoi(getenv("VLY_ATTN_IKEYS")) : 0;
-    p.attn_ikeys = (env_ik >= 16 && env_ik <= 256 && env_ik % 16 == 0) ? env_ik : 0;
-  }
-  p.sample = kv->d_sample;
-  p.l2_hint = kv->l2_hint;
-  {
-    static const bool want = getenv("VLY_MEGA_DBG") != nullptr;
-    p.dbg = want ? kv->dbg : nullptr;
-    g_mega_dbg = kv->dbg;
-  }
-  size_t x_bytes, misc;
-  mega_smem_layout(g, bmax, &x_bytes, &misc);
-  const size_t stage_b = (size_t)kv->stage_bytes;
-  int n_stages = (int)(((long long)kMegaSmem - (long long)x_bytes - (long long)misc) / (long long)stage_b);
-  if (n_stages > MegaCfg::MAX_STAGES) n_stages = MegaCfg::MAX_STAGES;
-  {
-    // depth of the ring and number of stages kept in flight: see pick_phase_geometry.  VLY_MEGA_STAGES / VLY_MEGA_INFLIGHT override.
-    static const int want = getenv("VLY_MEGA_STAGES") ? atoi(getenv("VLY_MEGA_STAGES")) : 0;
-    const int cap = want > 0 ? want : 4;            // deeper rings made every grid barrier slower (see pick_phase_geometry)
-    if (n_stages > cap) n_stages = cap;
-    static const int inflight = getenv("VLY_MEGA_INFLIGHT") ? atoi(getenv("VLY_MEGA_INFLIGHT")) : 0;
-    p.n_inflight = inflight > 0 ? inflight : n_stages;                        // (PhaseDesc::inflight is the per-phase value)
-    if (p.n_inflight > n_stages) p.n_inflight = n_stages;
-  }
-  if (n_stages < 2) return fail(VLY_ERR_INVALID, "decode: activations (B=%d, K=%d) leave no room for the weight ring", B, p.Kmax);
-  p.n_stages = n_stages;
-  p.stage_bytes = (int)stage_b;
-  const size_t smem = (size_t)n_stages * stage_b + x_bytes + misc;
-  void* args[] = {&p};
+  const int bmax = kv->B <= 1 ? 1 : (kv->B <= 2 ? 2 : 4);
+  void* args[] = {&kv->mega};
   cudaError_t e;
-#define VLY_MEGA_CASE(BM)                                                                                               \
-  {                                                                                                                     \
-    TRY(ensure_smem_attr(c->cfg.device, decode_step_kernel<BM>, smem));                                                 \
-    e = cudaLaunchCooperativeKernel((void*)decode_step_kernel<BM>, dim3(c->num_sms), dim3(MegaCfg::THREADS), args, smem, st); \
+#define VLY_MEGA_CASE(BM)                                                                                                          \
+  {                                                                                                                                \
+    TRY(ensure_smem_attr(c->cfg.device, decode_step_kernel<BM>, kv->mega_smem));                                                   \
+    e = cudaLaunchCooperativeKernel((void*)decode_step_kernel<BM>, dim3(c->num_sms), dim3(MegaCfg::THREADS), args, kv->mega_smem, st); \
   }
   if (bmax == 1) VLY_MEGA_CASE(1)
   else if (bmax == 2) VLY_MEGA_CASE(2)
@@ -1695,7 +1668,7 @@ static int launch_decode_mega(vly_ctx* c, vly_kv* kv, cudaStream_t st) {
 }
 
 static int enqueue_full_step(vly_ctx* c, vly_kv* kv, cudaStream_t st) {
-  if (decode_mode() == 2 && kv->B <= 4) return launch_decode_mega(c, kv, st);
+  if (kv->B <= 4) return launch_decode_mega(c, kv, st);
   for (int b0 = 0; b0 < kv->B; b0 += 4) {
     const int nb = (kv->B - b0) < 4 ? (kv->B - b0) : 4;
     TRY(enqueue_decode_step(c, kv, b0, nb, b0 + 4 >= kv->B, st));
@@ -1762,8 +1735,7 @@ static int capture_steps(vly_ctx* c, vly_kv* kv, int n, cudaGraphExec_t* out) {
 static int build_graph(vly_ctx* c, vly_kv* kv) {
   if (kv->graph) return VLY_OK;
   TRY(capture_steps(c, kv, 1, &kv->graph));
-  static const bool multi = getenv("VLY_GRAPH_STEPS1") == nullptr;
-  if (multi) TRY(capture_steps(c, kv, kGraphSteps, &kv->graph_n));
+  TRY(capture_steps(c, kv, kGraphSteps, &kv->graph_n));
   return VLY_OK;
 }
 

@@ -118,17 +118,6 @@ VLY_DEVINL uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
   return d;
 }
 
-// ------------------------------------------------------------------------------------------
-// vector global access
-// ------------------------------------------------------------------------------------------
-VLY_DEVINL uint4 ldg_nc_v4(const void* p) {
-  uint4 r;
-  asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];\n"
-               : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
-               : "l"(p));
-  return r;
-}
-
 VLY_DEVINL float fast_exp2(float x) {  // MUFU.EX2; exp2(-inf) = 0
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));

@@ -1,4 +1,5 @@
-// Decode path, generation 2: HBM-bound weight streaming with TMA bulk copies and mbarriers.
+// Per-op decode kernels (B > 4 in groups of 4, and the prefill's last-token logits): HBM-bound weight streaming with TMA
+// bulk copies and mbarriers.
 //
 //   gemv_ring_kernel : y[b,n] = sum_k x[b,k] W[n,k] for B <= 4.  One persistent CTA per SM.  A producer warp streams the
 //                      weight rows through a shared-memory ring with 1-D bulk (TMA) copies -- 8 rows x 2048 columns (32 KB)
@@ -14,9 +15,60 @@
 //                      bulk-copied to shared memory before griddepcontrol.wait; only q and the newest key/value wait.
 #pragma once
 #include "common.cuh"
-#include "simt_kernels.cuh"
 
 namespace vly {
+
+enum GemvMode : int {
+  GEMV_QKV_ROPE = 0,   // RMSNorm fold + RoPE + KV-cache append (HF:modeling_llama.py:262-270)
+  GEMV_RESIDUAL = 1,   // y + residual -> bf16 (o_proj, down_proj)
+  GEMV_SWIGLU = 2,     // RMSNorm fold + silu(g)*u with interleaved (g,u) rows
+  GEMV_LOGITS = 3,     // RMSNorm fold + fp32 logits (+ fused greedy argmax, model_worker.py:390-391)
+};
+
+struct GemvParams {
+  int N, K, B;
+  const __nv_bfloat16* W;
+  const __nv_bfloat16* x;       // [B, K], row stride ldx elements
+  long long ldx;
+  float eps;
+  __nv_bfloat16* out;           // QKV: q [B,H]; RESIDUAL: [B,N]; SWIGLU: [B,N/2]
+  const __nv_bfloat16* res;     // RESIDUAL: [B,N]
+  const float2* rope;           // [max_pos, 64]
+  const int* seq_len;           // device scalar: tokens already in the cache (== position of the new token)
+  int H, nH, Smax;
+  __nv_bfloat16* kcache;        // [B, nH, Smax, 128] (this layer)
+  __nv_bfloat16* vcache;
+  float* logits;                // [B, N] or nullptr
+  float* part_val;              // [B, grid]
+  int* part_idx;                // [B, grid]
+  unsigned int* counter;
+  long long* next_tokens;       // [B]
+  long long* out_tokens;        // [B, out_stride] or nullptr
+  int out_stride;
+  int* step;                    // device scalar: decode step index (column of out_tokens)
+  int* seq_len_rw;              // incremented by the last CTA of the logits kernel (end of step)
+  int bump;                     // 1: this launch closes the step (advance *step and *seq_len_rw)
+};
+
+struct DecAttnParams {
+  int B, nH, H, Smax, nsplit;
+  const int* seq_len;               // tokens in the cache BEFORE this step; the new K/V were just appended at that index
+  const __nv_bfloat16* q;           // [B, H]  (interleaved RoPE order, matches the cache's K)
+  const __nv_bfloat16* kcache;      // [B, nH, Smax, 128]
+  const __nv_bfloat16* vcache;
+  float* part_o;                    // [B*nH, nsplit, 128]
+  float2* part_ml;                  // [B*nH, nsplit]
+  unsigned int* counters;           // [B*nH]
+  __nv_bfloat16* out;               // [B, H]
+  float scale_log2e;
+  const uint32_t* key_bits;         // [B, mask_words] bit k of row b = key k may be attended (attention_mask); never null
+  int mask_words;
+};
+
+// HF's 2-D attention_mask as one bit per cache position (vly_kv_set_key_mask); positions nobody masked are 1.
+__device__ __forceinline__ bool key_attendable(const uint32_t* __restrict__ bits, int k) {
+  return (__ldg(bits + (k >> 5)) >> (k & 31)) & 1u;
+}
 
 struct RingCfg {
   static constexpr int ROWS = 4;                          // rows per work unit: N/4 units balance to ~1% over the SMs

@@ -129,9 +129,7 @@ VLY_DEVINL void grid_sync_consumers(unsigned int* counter, unsigned int target, 
   asm volatile("bar.sync 2, 544;" ::: "memory");
 }
 
-// ------------------------------ attention phase (shared by both step kernels) ------------------------------
-// Runs on the 16 compute warps (cw = 0..15); no block-level barrier inside.
-// ------------------------------ attention phase (shared by both step kernels) ------------------------------
+// ------------------------------ attention phase ------------------------------
 // Runs on the 16 compute warps (cw = 0..15); no block-level barrier inside.
 // (A CTA-per-(sequence, head) variant with a shared-memory merge was measured at 13B, B = 4: slower -- one SM cannot keep enough
 //  K/V loads in flight from registers; spreading every head over all SMs wins despite the global-memory merge.)
@@ -329,7 +327,7 @@ VLY_DEVINL void mega_epilogue_prefetch(const StepParams& p, const PhaseDesc& d, 
   }
 }
 
-// ------------------------------ fused epilogue of one work unit (shared by both step kernels) ------------------------------
+// ------------------------------ fused epilogue of one work unit ------------------------------
 // Executed by the lanes < NV of the epilogue warp: lane = r * BMAX + b holds t = the finished dot product of weight row n = n0 + r
 // and batch row b.  pre0 / pre1: the operand prefetched before the unit completed (residual, or RoPE cos / sin).
 template <int BMAX, int NV>

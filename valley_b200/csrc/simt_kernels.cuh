@@ -1,6 +1,5 @@
-// SIMT kernels: layout / gather kernels around the tensor-core path, and the HBM-bound
-// single-token decode path (weight-streaming GEMVs with fused RMSNorm / RoPE / KV append /
-// SwiGLU / residual / argmax epilogues, split-KV attention).
+// SIMT kernels: layout / gather kernels around the tensor-core path, the per-op decode path's embedding
+// gather, cross-entropy and weight-upload conversions.
 #pragma once
 #include "common.cuh"
 
@@ -175,387 +174,6 @@ __global__ void decode_embed_kernel(const long long* __restrict__ tokens, const 
   id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
   for (int c = threadIdx.x * 8; c < H; c += blockDim.x * 8)
     *reinterpret_cast<uint4*>(x + (size_t)b * H + c) = *reinterpret_cast<const uint4*>(embed + (size_t)id * H + c);
-}
-
-// ============================================================================================
-// Decode GEMV family:  y[b, n] = sum_k x[b, k] * W[n, k],  B <= BMAX (1..4), W streamed once from HBM.
-// CTA = 256 threads; a work unit is 8 consecutive weight rows; every thread owns 16-byte K chunks
-// (chunk c -> thread c % 256), so a warp reads 512 contiguous bytes of each row.  x lives in shared
-// memory (bf16), read once per chunk and reused for the 8 rows.
-// ============================================================================================
-enum GemvMode : int {
-  GEMV_QKV_ROPE = 0,   // RMSNorm fold + RoPE + KV-cache append (HF:modeling_llama.py:262-270)
-  GEMV_RESIDUAL = 1,   // y + residual -> bf16 (o_proj, down_proj)
-  GEMV_SWIGLU = 2,     // RMSNorm fold + silu(g)*u with interleaved (g,u) rows
-  GEMV_LOGITS = 3,     // RMSNorm fold + fp32 logits (+ fused greedy argmax, model_worker.py:390-391)
-};
-
-struct GemvParams {
-  int N, K, B;
-  const __nv_bfloat16* W;
-  const __nv_bfloat16* x;       // [B, K], row stride ldx elements
-  long long ldx;
-  float eps;
-  __nv_bfloat16* out;           // QKV: q [B,H]; RESIDUAL: [B,N]; SWIGLU: [B,N/2]
-  const __nv_bfloat16* res;     // RESIDUAL: [B,N]
-  const float2* rope;           // [max_pos, 64]
-  const int* seq_len;           // device scalar: tokens already in the cache (== position of the new token)
-  int H, nH, Smax;
-  __nv_bfloat16* kcache;        // [B, nH, Smax, 128] (this layer)
-  __nv_bfloat16* vcache;
-  float* logits;                // [B, N] or nullptr
-  float* part_val;              // [B, grid]
-  int* part_idx;                // [B, grid]
-  unsigned int* counter;
-  long long* next_tokens;       // [B]
-  long long* out_tokens;        // [B, out_stride] or nullptr
-  int out_stride;
-  int* step;                    // device scalar: decode step index (column of out_tokens)
-  int* seq_len_rw;              // incremented by the last CTA of the logits kernel (end of step)
-  int bump;                     // 1: this launch closes the step (advance *step and *seq_len_rw)
-};
-
-template <int BMAX, int MODE>
-__global__ void __launch_bounds__(256, 2) gemv_kernel(const GemvParams p) {
-  extern __shared__ __align__(16) uint8_t gsm[];
-  __nv_bfloat16* xs = reinterpret_cast<__nv_bfloat16*>(gsm);                           // [BMAX, K]
-  float* red = reinterpret_cast<float*>(gsm + (size_t)BMAX * p.K * 2);                  // [2][8 warps][8][BMAX]
-  float* fin = red + 2 * 8 * 8 * BMAX;                                                  // [2][8][BMAX]
-  float* rstd_s = fin + 2 * 8 * BMAX;                                                   // [BMAX]
-  float* bestv = rstd_s + BMAX;                                                         // [BMAX]
-  int* besti = reinterpret_cast<int*>(bestv + BMAX);                                    // [BMAX]
-  __shared__ float wred[8][BMAX];
-  __shared__ int is_last;
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int chunks = p.K >> 3;
-
-  // ---- stage x in shared memory; RMSNorm statistics where the mode folds a norm ----
-  {
-    float sq[BMAX];
-#pragma unroll
-    for (int b = 0; b < BMAX; ++b) sq[b] = 0.f;
-    for (int c = tid; c < chunks; c += 256) {
-#pragma unroll
-      for (int b = 0; b < BMAX; ++b) {
-        uint4 w = make_uint4(0, 0, 0, 0);
-        if (b < p.B) w = *reinterpret_cast<const uint4*>(p.x + (size_t)b * p.ldx + c * 8);
-        *reinterpret_cast<uint4*>(xs + (size_t)b * p.K + c * 8) = w;
-        if constexpr (MODE != GEMV_RESIDUAL) {
-          const uint32_t ww[4] = {w.x, w.y, w.z, w.w};
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const float a = bf16_lo(ww[i]), bb = bf16_hi(ww[i]);
-            sq[b] += a * a + bb * bb;
-          }
-        }
-      }
-    }
-    if constexpr (MODE != GEMV_RESIDUAL) {
-#pragma unroll
-      for (int b = 0; b < BMAX; ++b) {
-        const float v = warp_sum(sq[b]);
-        if (lane == 0) wred[warp][b] = v;
-      }
-      __syncthreads();
-      if (tid < BMAX) {
-        float t = 0.f;
-        for (int w = 0; w < 8; ++w) t += wred[w][tid];
-        rstd_s[tid] = rsqrtf(t / p.K + p.eps);
-      }
-    }
-    if (tid < BMAX) {
-      bestv[tid] = -INFINITY;
-      besti[tid] = 0;
-    }
-    __syncthreads();
-  }
-
-  int pos = 0;
-  if constexpr (MODE == GEMV_QKV_ROPE) pos = *p.seq_len;
-
-  const int units = (p.N + 7) >> 3;
-  int par = 0;
-  for (int u = blockIdx.x; u < units; u += gridDim.x, par ^= 1) {
-    const int n0 = u * 8;
-    float acc[8][BMAX];
-#pragma unroll
-    for (int r = 0; r < 8; ++r)
-#pragma unroll
-      for (int b = 0; b < BMAX; ++b) acc[r][b] = 0.f;
-
-    const __nv_bfloat16* wbase = p.W + (size_t)n0 * p.K;
-    const int rows_ok = min(8, p.N - n0);
-#pragma unroll 2
-    for (int c = tid; c < chunks; c += 256) {
-      uint4 w[8];
-#pragma unroll
-      for (int r = 0; r < 8; ++r)
-        w[r] = (r < rows_ok) ? ldg_nc_v4(wbase + (size_t)r * p.K + c * 8) : make_uint4(0, 0, 0, 0);
-      float xf[BMAX][8];
-#pragma unroll
-      for (int b = 0; b < BMAX; ++b) {
-        const uint4 xv = *reinterpret_cast<const uint4*>(xs + (size_t)b * p.K + c * 8);
-        xf[b][0] = bf16_lo(xv.x); xf[b][1] = bf16_hi(xv.x); xf[b][2] = bf16_lo(xv.y); xf[b][3] = bf16_hi(xv.y);
-        xf[b][4] = bf16_lo(xv.z); xf[b][5] = bf16_hi(xv.z); xf[b][6] = bf16_lo(xv.w); xf[b][7] = bf16_hi(xv.w);
-      }
-#pragma unroll
-      for (int r = 0; r < 8; ++r) {
-        const float wf[8] = {bf16_lo(w[r].x), bf16_hi(w[r].x), bf16_lo(w[r].y), bf16_hi(w[r].y),
-                             bf16_lo(w[r].z), bf16_hi(w[r].z), bf16_lo(w[r].w), bf16_hi(w[r].w)};
-#pragma unroll
-        for (int b = 0; b < BMAX; ++b)
-#pragma unroll
-          for (int e = 0; e < 8; ++e) acc[r][b] = fmaf(wf[e], xf[b][e], acc[r][b]);
-      }
-    }
-    // ---- reduce over the 256 threads ----
-    float* redp = red + par * (8 * 8 * BMAX);
-#pragma unroll
-    for (int r = 0; r < 8; ++r)
-#pragma unroll
-      for (int b = 0; b < BMAX; ++b) {
-        const float v = warp_sum(acc[r][b]);
-        if (lane == 0) redp[(warp * 8 + r) * BMAX + b] = v;
-      }
-    __syncthreads();
-    float* finp = fin + par * (8 * BMAX);
-    if (tid < 8 * BMAX) {
-      float t = 0.f;
-#pragma unroll
-      for (int w = 0; w < 8; ++w) t += redp[w * 8 * BMAX + tid];   // tid == r*BMAX + b
-      finp[tid] = t;
-    }
-    __syncthreads();
-
-    // ---- fused epilogues ----
-    if constexpr (MODE == GEMV_RESIDUAL) {
-      if (tid < 8 * BMAX) {
-        const int r = tid / BMAX, b = tid % BMAX, n = n0 + r;
-        if (b < p.B && n < p.N) {
-          const float y = finp[tid] + __bfloat162float(p.res[(size_t)b * p.N + n]);
-          p.out[(size_t)b * p.N + n] = __float2bfloat16_rn(y);
-        }
-      }
-    } else if constexpr (MODE == GEMV_SWIGLU) {
-      if (tid < 4 * BMAX) {
-        const int j = tid / BMAX, b = tid % BMAX, n = n0 + 2 * j;
-        if (b < p.B && n + 1 < p.N) {
-          const float rs = rstd_s[b];
-          // HF rounds gate and up to bf16 before silu*mul (modeling_llama.py:182-184)
-          const float g = bf16_round(finp[(2 * j) * BMAX + b] * rs), uu = bf16_round(finp[(2 * j + 1) * BMAX + b] * rs);
-          p.out[(size_t)b * (p.N >> 1) + (n >> 1)] = __float2bfloat16_rn(bf16_round(g / (1.f + __expf(-g))) * uu);
-        }
-      }
-    } else if constexpr (MODE == GEMV_QKV_ROPE) {
-      if (tid < 4 * BMAX) {
-        const int j = tid / BMAX, b = tid % BMAX, n = n0 + 2 * j;
-        if (b < p.B && n + 1 < p.N) {
-          const float rs = rstd_s[b];
-          float x0 = finp[(2 * j) * BMAX + b] * rs, x1 = finp[(2 * j + 1) * BMAX + b] * rs;
-          const int which = n / p.H, nh = n - which * p.H, head = nh >> 7, cidx = nh & 127;
-          if (which < 2) {
-            const float2 cs = p.rope[(size_t)pos * 64 + (cidx >> 1)];
-            const float a = x0 * cs.x - x1 * cs.y, c2 = x1 * cs.x + x0 * cs.y;
-            x0 = a;
-            x1 = c2;
-          }
-          __nv_bfloat16* dst;
-          if (which == 0) dst = p.out + (size_t)b * p.H + nh;
-          else dst = ((which == 1) ? p.kcache : p.vcache) + (((size_t)b * p.nH + head) * p.Smax + pos) * 128 + cidx;
-          *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(x0, x1);
-        }
-      }
-    } else {  // GEMV_LOGITS
-      if (tid < 8 * BMAX) {
-        const int r = tid / BMAX, b = tid % BMAX, n = n0 + r;
-        if (b < p.B && n < p.N) {
-          const float y = finp[tid] * rstd_s[b];
-          finp[tid] = y;
-          if (p.logits != nullptr) p.logits[(size_t)b * p.N + n] = y;
-        }
-      }
-      __syncwarp();
-      // rows of a unit are finalised by 8*BMAX <= 32 threads of warp 0; one thread per b scans them in index order
-      if (tid < BMAX && tid < p.B) {
-        for (int r = 0; r < 8 && n0 + r < p.N; ++r) {
-          const float y = finp[r * BMAX + tid];
-          if (y > bestv[tid]) {
-            bestv[tid] = y;
-            besti[tid] = n0 + r;
-          }
-        }
-      }
-    }
-  }
-
-  if constexpr (MODE == GEMV_LOGITS) {
-    __syncthreads();
-    if (tid < p.B) {
-      p.part_val[(size_t)tid * gridDim.x + blockIdx.x] = bestv[tid];
-      p.part_idx[(size_t)tid * gridDim.x + blockIdx.x] = besti[tid];
-    }
-    __threadfence();
-    __syncthreads();
-    if (tid == 0) is_last = (atomicAdd(p.counter, 1u) == gridDim.x - 1);
-    __syncthreads();
-    if (is_last) {
-      __threadfence();
-      if (warp < p.B) {   // one warp per batch row
-        const int b = warp;
-        float bv = -INFINITY;
-        int bi = 0x7fffffff;
-        for (int g = lane; g < (int)gridDim.x; g += 32) {
-          const float v = __ldcg(p.part_val + (size_t)b * gridDim.x + g);
-          const int i = __ldcg(p.part_idx + (size_t)b * gridDim.x + g);
-          if (v > bv || (v == bv && i < bi)) { bv = v; bi = i; }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-          const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-          const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-          if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-        }
-        if (lane == 0) {
-          p.next_tokens[b] = bi;
-          if (p.out_tokens != nullptr) p.out_tokens[(size_t)b * p.out_stride + *p.step] = bi;
-        }
-      }
-      __syncthreads();
-      if (tid == 0) {
-        *p.counter = 0;
-        if (p.bump) {
-          *p.step += 1;
-          *p.seq_len_rw += 1;
-        }
-      }
-    }
-  }
-}
-
-// ============================================================================================
-// Decode attention: one new query per (b, head) against the cache (HF:modeling_llama.py:199-222 with S_q = 1).
-// grid (B*nH, nsplit), 128 threads.  Split-KV partials are merged by the last CTA of each (b, head).
-// ============================================================================================
-struct DecAttnParams {
-  int B, nH, H, Smax, nsplit;
-  const int* seq_len;               // tokens in the cache BEFORE this step; the new K/V were just appended at that index
-  const __nv_bfloat16* q;           // [B, H]  (interleaved RoPE order, matches the cache's K)
-  const __nv_bfloat16* kcache;      // [B, nH, Smax, 128]
-  const __nv_bfloat16* vcache;
-  float* part_o;                    // [B*nH, nsplit, 128]
-  float2* part_ml;                  // [B*nH, nsplit]
-  unsigned int* counters;           // [B*nH]
-  __nv_bfloat16* out;               // [B, H]
-  float scale_log2e;
-  const uint32_t* key_bits;         // [B, mask_words] bit k of row b = key k may be attended (attention_mask); never null
-  int mask_words;
-};
-
-// HF's 2-D attention_mask as one bit per cache position (vly_kv_set_key_mask); positions nobody masked are 1.
-__device__ __forceinline__ bool key_attendable(const uint32_t* __restrict__ bits, int k) {
-  return (__ldg(bits + (k >> 5)) >> (k & 31)) & 1u;
-}
-
-__global__ void __launch_bounds__(128) decode_attention_kernel(const DecAttnParams p) {
-  extern __shared__ __align__(16) float dsm[];
-  float* sc = dsm;                                  // [per]
-  __shared__ float redg[8][128];
-  __shared__ float wr[4];
-  __shared__ int is_last;
-  const int bh = blockIdx.x, split = blockIdx.y;
-  const int b = bh / p.nH, h = bh % p.nH;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int len = *p.seq_len + 1;
-  const int per = (len + p.nsplit - 1) / p.nsplit;
-  const int k0 = split * per, k1 = min(len, k0 + per);
-  const int nk = max(0, k1 - k0);
-  const __nv_bfloat16* kb = p.kcache + ((size_t)bh * p.Smax) * 128;
-  const __nv_bfloat16* vb = p.vcache + ((size_t)bh * p.Smax) * 128;
-
-  // q chunk of this lane (8 dims)
-  const int hl = lane & 15;
-  float qf[8];
-  {
-    const uint4 w = *reinterpret_cast<const uint4*>(p.q + (size_t)b * p.H + h * 128 + hl * 8);
-    qf[0] = bf16_lo(w.x); qf[1] = bf16_hi(w.x); qf[2] = bf16_lo(w.y); qf[3] = bf16_hi(w.y);
-    qf[4] = bf16_lo(w.z); qf[5] = bf16_hi(w.z); qf[6] = bf16_lo(w.w); qf[7] = bf16_hi(w.w);
-  }
-  // ---- scores ----
-  for (int i0 = warp * 2; i0 < nk; i0 += 8) {   // warp-uniform trip count (two keys per warp iteration)
-    const int i = i0 + (lane >> 4);
-    const bool ok = i < nk;
-    uint4 w = make_uint4(0, 0, 0, 0);
-    if (ok) w = ldg_nc_v4(kb + (size_t)(k0 + i) * 128 + hl * 8);
-    float d = qf[0] * bf16_lo(w.x) + qf[1] * bf16_hi(w.x) + qf[2] * bf16_lo(w.y) + qf[3] * bf16_hi(w.y) +
-              qf[4] * bf16_lo(w.z) + qf[5] * bf16_hi(w.z) + qf[6] * bf16_lo(w.w) + qf[7] * bf16_hi(w.w);
-    d += __shfl_xor_sync(0xffffffffu, d, 8);
-    d += __shfl_xor_sync(0xffffffffu, d, 4);
-    d += __shfl_xor_sync(0xffffffffu, d, 2);
-    d += __shfl_xor_sync(0xffffffffu, d, 1);
-    if (ok && hl == 0) sc[i] = key_attendable(p.key_bits + (size_t)b * p.mask_words, k0 + i) ? d * p.scale_log2e : -INFINITY;
-  }
-  __syncthreads();
-  float m = -INFINITY;
-  for (int i = tid; i < nk; i += 128) m = fmaxf(m, sc[i]);
-  m = warp_max(m);
-  if (lane == 0) wr[warp] = m;
-  __syncthreads();
-  m = fmaxf(fmaxf(wr[0], wr[1]), fmaxf(wr[2], wr[3]));
-  __syncthreads();
-  float l = 0.f;
-  for (int i = tid; i < nk; i += 128) {
-    const float e = sc[i] > -INFINITY ? fast_exp2(sc[i] - m) : 0.f;   // masked key (m itself may be -inf)
-    sc[i] = e;
-    l += e;
-  }
-  l = warp_sum(l);
-  if (lane == 0) wr[warp] = l;
-  __syncthreads();
-  l = wr[0] + wr[1] + wr[2] + wr[3];
-  // ---- P V : 16 threads cover one value row (8 dims each), 8 keys in flight ----
-  {
-    const int g = tid >> 4, dl = tid & 15;
-    float o[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    for (int i = g; i < nk; i += 8) {
-      const float pw = sc[i];
-      const uint4 w = ldg_nc_v4(vb + (size_t)(k0 + i) * 128 + dl * 8);
-      o[0] = fmaf(pw, bf16_lo(w.x), o[0]); o[1] = fmaf(pw, bf16_hi(w.x), o[1]);
-      o[2] = fmaf(pw, bf16_lo(w.y), o[2]); o[3] = fmaf(pw, bf16_hi(w.y), o[3]);
-      o[4] = fmaf(pw, bf16_lo(w.z), o[4]); o[5] = fmaf(pw, bf16_hi(w.z), o[5]);
-      o[6] = fmaf(pw, bf16_lo(w.w), o[6]); o[7] = fmaf(pw, bf16_hi(w.w), o[7]);
-    }
-#pragma unroll
-    for (int e = 0; e < 8; ++e) redg[g][dl * 8 + e] = o[e];
-  }
-  __syncthreads();
-  float ot = 0.f;
-#pragma unroll
-  for (int g = 0; g < 8; ++g) ot += redg[g][tid];
-
-  p.part_o[((size_t)bh * p.nsplit + split) * 128 + tid] = ot;
-  if (tid == 0) p.part_ml[(size_t)bh * p.nsplit + split] = make_float2(m, l);
-  __threadfence();
-  __syncthreads();
-  if (tid == 0) is_last = (atomicAdd(p.counters + bh, 1u) == (unsigned)p.nsplit - 1);
-  __syncthreads();
-  if (is_last) {
-    __threadfence();
-    float M = -INFINITY;
-    for (int s = 0; s < p.nsplit; ++s) M = fmaxf(M, __ldcg(&p.part_ml[(size_t)bh * p.nsplit + s].x));
-    float L = 0.f, acc = 0.f;
-    for (int s = 0; s < p.nsplit; ++s) {
-      const float ms = __ldcg(&p.part_ml[(size_t)bh * p.nsplit + s].x);
-      const float ls = __ldcg(&p.part_ml[(size_t)bh * p.nsplit + s].y);
-      if (ls > 0.f) {
-        const float w = fast_exp2(ms - M);
-        L += ls * w;
-        acc += __ldcg(p.part_o + ((size_t)bh * p.nsplit + s) * 128 + tid) * w;
-      }
-    }
-    p.out[(size_t)b * p.H + h * 128 + tid] = __float2bfloat16_rn(L > 0.f ? acc / L : 0.f);
-    if (tid == 0) p.counters[bh] = 0;
-  }
 }
 
 // ============================================================================================
