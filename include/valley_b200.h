@@ -13,7 +13,7 @@
  *   - "dev" pointers are CUDA device pointers owned by the caller (e.g. a torch tensor's data_ptr());
  *     the library owns only its packed weights, workspace and KV caches (tied to vly_ctx / vly_kv).
  *   - calls are stream-ordered on the cudaStream_t passed in (void* stream; NULL = legacy default stream).
- *   - there is NO CPU fallback: without a CUDA device of compute capability 10.x vly_create fails.
+ *   - there is NO CPU fallback: without a CUDA device of compute capability 9.x vly_create fails.
  *   - hot calls do not allocate once the workspace has grown to the largest shapes seen, so the decode
  *     step is captured in a CUDA graph (vly_generate_greedy).
  *   - thread safety: a vly_ctx serialises its workspace-using calls with an internal mutex
@@ -92,7 +92,9 @@ int vly_vit_encode(vly_ctx* ctx, const void* pixels_dev, int pixel_dtype, int n_
  *   vly_gather_create     : allocate this rank's gather buffer [rows_total, 1024] bf16 (+flags) and export its 64-byte CUDA IPC handle
  *   vly_gather_open_peers : map all ranks' buffers (handles gathered by the caller, e.g. torch.distributed.all_gather_object)
  *   vly_vit_encode_gather : encode n_frames local frames that start at global frame index frame_offset; on return (stream
- *                           order) the local gather buffer holds the features of ALL ranks' frames */
+ *                           order) the local gather buffer holds the features of ALL ranks' frames
+ * vly_destroy unmaps the peers' buffers and frees this rank's, which the peers write into: every rank must have finished its
+ * last vly_vit_encode_gather before any rank destroys its context. */
 int vly_gather_create(vly_ctx* ctx, int64_t rows_total, void** local_buf_dev, void* ipc_handle_out_64B);
 int vly_gather_open_peers(vly_ctx* ctx, const void* handles_64B_each, int world, int rank);
 int vly_vit_encode_gather(vly_ctx* ctx, const void* pixels_dev, int pixel_dtype, int n_frames, int frame_offset, int select_layer,
@@ -208,6 +210,9 @@ int vly_generate(vly_ctx* ctx, vly_kv* kv, const int64_t* first_tokens_dev, int 
 
 /* ---- introspection for bench / tests ---- */
 int vly_kernel_launch_count(vly_ctx* ctx, int64_t* out);   /* kernels launched by this ctx so far */
+/* bytes of device memory and of pinned host memory the library holds right now, summed over every context and KV cache of
+ * the process (packed and staged weights, workspace, caches, gather buffers) */
+int vly_held_bytes(int64_t* device_bytes, int64_t* pinned_bytes);
 int vly_num_sms(vly_ctx* ctx, int* out);
 
 /* in-kernel cycle counters of kv's last decode step (tools/bench_decode.py): copies n int64 values to host_out.  Only a

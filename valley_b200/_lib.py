@@ -83,6 +83,7 @@ SIGNATURES = {
     "vly_sample_logits": (_i, [_vp, _vp, _vp, _p(VlySampling), _vp, _vp]),
     "vly_generate": (_i, [_vp, _vp, _vp, _i, _vp, _p(VlySampling), _vp, _vp]),
     "vly_kernel_launch_count": (_i, [_vp, _p(_i64)]),
+    "vly_held_bytes": (_i, [_p(_i64), _p(_i64)]),
     "vly_num_sms": (_i, [_vp, _p(_i)]),
     "vly_kv_debug_counters": (_i, [_vp, _vp, _i]),
     "vly_set_error_": (None, [C.c_char_p]),

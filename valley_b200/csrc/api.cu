@@ -4,12 +4,14 @@
 #include <cuda.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -57,33 +59,67 @@ extern "C" const char* vly_version(void) { return "valley_b200 0.1 (sm_90a)"; }
 // ------------------------------------------------------------------------------------------------
 // data structures
 // ------------------------------------------------------------------------------------------------
-struct Buf {
+// Bytes held by all live Mem objects of the process: [0] device memory, [1] pinned host memory (vly_held_bytes).
+static std::atomic<int64_t> g_held_bytes[2];
+
+// One allocation of the library: device memory, or pinned host memory (which the device can address too).  Move-only; the
+// memory is freed when its owner is destroyed.  Its constructor and destructor are the only code that updates g_held_bytes.
+struct Mem {
   void* p = nullptr;
   size_t bytes = 0;
+  bool pinned = false;
+  Mem() = default;
+  Mem(void* q, size_t n, bool host) : p(q), bytes(n), pinned(host) { g_held_bytes[pinned] += (int64_t)bytes; }
+  Mem(Mem&& o) noexcept { swap(o); }
+  Mem& operator=(Mem&& o) noexcept {
+    Mem t(std::move(o));
+    swap(t);  // t leaves with what this held
+    return *this;
+  }
+  ~Mem() {
+    if (!p) return;
+    if (pinned) cudaFreeHost(p);
+    else cudaFree(p);
+    g_held_bytes[pinned] -= (int64_t)bytes;
+  }
+  void swap(Mem& o) noexcept {
+    std::swap(p, o.p);
+    std::swap(bytes, o.bytes);
+    std::swap(pinned, o.pinned);
+  }
+  // replaces what this holds by n new bytes; the old allocation is freed first
+  int alloc(size_t n, bool host = false) {
+    *this = Mem();
+    void* q = nullptr;
+    if (host) CK(cudaHostAlloc(&q, n, cudaHostAllocMapped));
+    else CK(cudaMalloc(&q, n));
+    *this = Mem(q, n, host);
+    return VLY_OK;
+  }
 };
-static int ensure(Buf& b, size_t bytes) {
-  if (b.bytes >= bytes) return VLY_OK;
-  if (b.p) CK(cudaFree(b.p));
-  b.p = nullptr;
-  b.bytes = 0;
-  CK(cudaMalloc(&b.p, bytes));
-  b.bytes = bytes;
-  return VLY_OK;
-}
+// a Mem that reads as a T*
+template <typename T>
+struct Owned : Mem {
+  operator T*() const { return static_cast<T*>(p); }
+  T* operator->() const { return static_cast<T*>(p); }
+};
+
+// grow-only workspace
+static int ensure(Mem& b, size_t bytes) { return b.bytes >= bytes ? VLY_OK : b.alloc(bytes); }
 
 struct Staged {
   std::vector<int64_t> shape;
-  void* dev = nullptr;
+  Mem mem;
   bool is_f32 = false;  // vectors are kept as fp32 holding bf16-rounded values; matrices as bf16
   int64_t numel = 0;
 };
 
 struct VitLayerW {
-  bf16 *wqkv, *wo, *w1, *w2;
-  float *qkv_cs, *qkv_b, *bo, *c1, *b1, *b2;
+  Owned<bf16> wqkv, wo, w1, w2;
+  Owned<float> qkv_cs, qkv_b, bo, c1, b1, b2;
 };
 struct LlamaLayerW {
-  bf16 *wqkv, *wo, *wgu, *wdown;
+  Owned<bf16> wqkv, wo, wgu, wdown;
 };
 
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -98,44 +134,50 @@ struct vly_ctx {
   std::map<std::string, Staged> staged;
   bool finalized = false;
   bool has_vit = false, has_llm = false;
-  std::vector<void*> owned;  // every packed weight allocation
   // ViT
   int kpad = 0;
-  bf16* patch_w = nullptr;
-  float *cls = nullptr, *pos = nullptr, *pre_g = nullptr, *pre_b = nullptr;
+  Owned<bf16> patch_w;
+  Owned<float> cls, pos, pre_g, pre_b;
   std::vector<VitLayerW> vit;
-  bf16* proj_w = nullptr;
-  float* proj_b = nullptr;
+  Owned<bf16> proj_w;
+  Owned<float> proj_b;
   // LLaMA
-  bf16* embed = nullptr;
+  Owned<bf16> embed;
   std::vector<LlamaLayerW> layers;
-  bf16* lm_head = nullptr;
-  float2* rope = nullptr;
+  Owned<bf16> lm_head;
+  Owned<float2> rope;
   // workspace
-  Buf w_col, w_patch, w_qkv, w_ctx, w_h, w_stats, w_pool, w_x, w_q, w_attn, w_hb, w_pstats;
+  Mem w_col, w_patch, w_qkv, w_ctx, w_h, w_stats, w_pool, w_x, w_q, w_attn, w_hb, w_pstats;
   cudaStream_t cap_stream = nullptr;
   int64_t launches = 0;
   // fused all-gather state
-  bf16* g_buf = nullptr;          // [g_rows, vit_hidden] + flags
+  Owned<bf16> g_buf;              // [g_rows, vit_hidden] + flags
   int64_t g_rows = 0;
   int* g_flags = nullptr;
-  bf16* g_peer_buf[8] = {};
+  bf16* g_peer_buf[8] = {};       // g_buf for this rank, CUDA IPC mappings of the other ranks' buffers
   int* g_peer_flags[8] = {};
   int g_world = 0, g_rank = 0, g_epoch = 0;
-  int* g_timeout = nullptr;       // pinned + mapped: set by gather_wait_kernel when a peer never signalled; read by the host
-  Buf w_xlocal;
+  Owned<int> g_timeout;           // pinned + mapped: set by gather_wait_kernel when a peer never signalled; read by the host
+  Mem w_xlocal;
   // pooling variants (valley_model.py:40-52, :205-213)
-  float* pool_U = nullptr;                     // temporal_importance: W_proj^T w_pool, [256, vit_hidden] fp32
+  Owned<float> pool_U;                         // temporal_importance: W_proj^T w_pool, [256, vit_hidden] fp32
   struct DeltaW {                              // temporal_transformer: one post-LN nn.TransformerEncoderLayer + position_matrix
-    bf16 *in_w = nullptr, *out_w = nullptr, *l1_w = nullptr, *l2_w = nullptr, *pos = nullptr;
-    float *in_b = nullptr, *out_b = nullptr, *l1_b = nullptr, *l2_b = nullptr, *n1_g = nullptr, *n1_b = nullptr, *n2_g = nullptr, *n2_b = nullptr;
+    Owned<bf16> in_w, out_w, l1_w, l2_w, pos;
+    Owned<float> in_b, out_b, l1_b, l2_b, n1_g, n1_b, n2_g, n2_b;
     int ffn = 0, max_pos = 0;
   } delta;
-  Buf w_score, w_pall, w_xp, w_dkv, w_dq, w_datt, w_dx1, w_df1, w_dx2;
+  Mem w_score, w_pall, w_xp, w_dkv, w_dq, w_datt, w_dx1, w_df1, w_dx2;
   // frame preprocessing: strip + coefficient tables of the last geometry seen
-  Buf w_strip, w_tables;
+  Mem w_strip, w_tables;
   int pre_H = 0, pre_W = 0;
   PreprocParams pre = {};
+
+  // (runs before the members above are freed)
+  ~vly_ctx() {
+    for (bf16* b : g_peer_buf)
+      if (b && b != g_buf) cudaIpcCloseMemHandle(b);
+    if (cap_stream) cudaStreamDestroy(cap_stream);
+  }
 };
 
 struct vly_kv;
@@ -143,32 +185,32 @@ static int sync_len(vly_kv* kv);
 struct vly_kv {
   vly_ctx* ctx;
   int B, Smax;
-  bf16* cache = nullptr;  // [L][2][B][nH][Smax][128]
+  Owned<bf16> cache;  // [L][2][B][nH][Smax][128]
   int host_len = 0;
   bool len_dirty = false;   // a stop token may have ended vly_generate early: host_len is re-read from the device on next use
-  int* h_len = nullptr;     // pinned: d_len is copied here on the generating stream, len_event marks the copy
+  Owned<int> h_len;         // pinned: d_len is copied here on the generating stream, len_event marks the copy
   cudaEvent_t len_event = nullptr;
-  int* d_len = nullptr;   // device scalar
+  Owned<int> d_len;       // device scalar
   int* d_step = nullptr;
   // decode workspace
-  bf16 *x = nullptr, *q = nullptr, *attn = nullptr, *hb = nullptr;
-  float* part_o = nullptr;
-  float2* part_ml = nullptr;
-  unsigned int* counters = nullptr;   // [B*nH] + 1 (argmax)
-  float* part_val = nullptr;          // [B, SMs]: per-CTA arg-max partials
-  int* part_idx = nullptr;
-  float* logits = nullptr;            // [B, V]
-  long long* cur_tokens = nullptr;    // [B]
-  long long* gen_tokens = nullptr;    // [B, Smax]
+  Owned<bf16> x, q, attn, hb;
+  Owned<float> part_o;
+  Owned<float2> part_ml;
+  Owned<unsigned int> counters;       // [B*nH] + 1 (argmax)
+  Owned<float> part_val;              // [B, SMs]: per-CTA arg-max partials
+  Owned<int> part_idx;
+  Owned<float> logits;                // [B, V]
+  Owned<long long> cur_tokens;        // [B]
+  Owned<long long> gen_tokens;        // [B, Smax]
   int nsplit = 1;
   // persistent decode kernel (B <= 4): the whole launch, fixed by vly_kv_create
-  PhaseDesc* d_phases = nullptr;
+  Owned<PhaseDesc> d_phases;
   StepParams mega = {};
   size_t mega_smem = 0;
-  long long* dbg = nullptr;           // [SMs][32] cycle counters (StepParams::dbg); allocated only with VLY_MEGA_DBG
-  SampleState* d_sample = nullptr;    // token selection state read by every decode step (sampling.cuh)
+  Owned<long long> dbg;               // [SMs][32] cycle counters (StepParams::dbg); allocated only with VLY_MEGA_DBG
+  Owned<SampleState> d_sample;        // token selection state read by every decode step (sampling.cuh)
   bool sample_dirty = false;          // device state is not the plain-greedy default
-  uint32_t* key_bits = nullptr;       // [B, Smax/32] attention_mask bits (1 = attend); all ones unless vly_kv_set_key_mask
+  Owned<uint32_t> key_bits;           // [B, Smax/32] attention_mask bits (1 = attend); all ones unless vly_kv_set_key_mask
   bool masked = false;
   int mask_words() const { return Smax / 32; }
   cudaGraphExec_t graph = nullptr;     // one decode step
@@ -177,6 +219,13 @@ struct vly_kv {
   size_t layer_stride() const { return (size_t)2 * B * ctx->cfg.num_attention_heads * Smax * 128; }
   bf16* k_layer(int l) const { return cache + (size_t)l * layer_stride(); }
   bf16* v_layer(int l) const { return k_layer(l) + layer_stride() / 2; }
+
+  // (runs before the buffers the graphs and the event refer to are freed)
+  ~vly_kv() {
+    if (graph) cudaGraphExecDestroy(graph);
+    if (graph_n) cudaGraphExecDestroy(graph_n);
+    if (len_event) cudaEventDestroy(len_event);
+  }
 };
 
 // after an eos-terminated vly_generate only the device knows how many steps ran (one blocking 4-byte read, off the hot path)
@@ -186,7 +235,7 @@ static int sync_len(vly_kv* kv) {
   if (!kv->len_dirty) return VLY_OK;
   CK(cudaSetDevice(kv->ctx->cfg.device));
   CK(cudaEventSynchronize(kv->len_event));
-  kv->host_len = *reinterpret_cast<volatile int*>(kv->h_len);
+  kv->host_len = *reinterpret_cast<volatile int*>(kv->h_len.p);
   kv->len_dirty = false;
   return VLY_OK;
 }
@@ -405,36 +454,23 @@ extern "C" int vly_create(const vly_config* cfg, vly_ctx** out) {
   if (cfg->intermediate_size % 64) return fail(VLY_ERR_INVALID, "vly_create: intermediate_size must be a multiple of 64");
   if (cfg->vit_hidden != 1024 || cfg->vit_hidden / cfg->vit_heads != 64 || cfg->vit_mlp % 256)
     return fail(VLY_ERR_INVALID, "vly_create: vision tower must be ViT-L width (1024, head_dim 64); the reference hard-codes 1024 (valley_model.py:192)");
-  vly_ctx* c = new vly_ctx();
+  auto c = std::make_unique<vly_ctx>();
   c->cfg = *cfg;
   c->num_sms = prop.multiProcessorCount;
   cudaDriverEntryPointQueryResult qres;
   void* fn = nullptr;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || fn == nullptr) {
-    delete c;
+  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || fn == nullptr)
     return fail(VLY_ERR_CUDA, "vly_create: cuTensorMapEncodeTiled entry point not found");
-  }
   c->encode = (PFN_encodeTiled)fn;
-  if (cudaStreamCreateWithFlags(&c->cap_stream, cudaStreamNonBlocking) != cudaSuccess) {
-    delete c;
+  if (cudaStreamCreateWithFlags(&c->cap_stream, cudaStreamNonBlocking) != cudaSuccess)
     return fail(VLY_ERR_CUDA, "vly_create: cudaStreamCreate failed");
-  }
-  *out = c;
+  *out = c.release();
   return VLY_OK;
 }
 
 extern "C" void vly_destroy(vly_ctx* c) {
   if (!c) return;
   cudaSetDevice(c->cfg.device);
-  for (auto& kvp : c->staged) cudaFree(kvp.second.dev);
-  for (void* p : c->owned) cudaFree(p);
-  Buf* bufs[] = {&c->w_col, &c->w_patch, &c->w_qkv, &c->w_ctx, &c->w_h, &c->w_stats, &c->w_pool, &c->w_x, &c->w_q, &c->w_attn, &c->w_hb, &c->w_pstats,
-                 &c->w_xlocal, &c->w_score, &c->w_pall, &c->w_xp, &c->w_dkv, &c->w_dq, &c->w_datt, &c->w_dx1, &c->w_df1, &c->w_dx2, &c->w_strip,
-                 &c->w_tables};
-  for (Buf* b : bufs)
-    if (b->p) cudaFree(b->p);
-  if (c->cap_stream) cudaStreamDestroy(c->cap_stream);
-  if (c->g_timeout) cudaFreeHost(c->g_timeout);
   delete c;
 }
 
@@ -446,6 +482,12 @@ extern "C" int vly_num_sms(vly_ctx* c, int* out) {
 extern "C" int vly_kernel_launch_count(vly_ctx* c, int64_t* out) {
   if (!c || !out) return fail(VLY_ERR_INVALID, "null");
   *out = c->launches;
+  return VLY_OK;
+}
+extern "C" int vly_held_bytes(int64_t* device_bytes, int64_t* pinned_bytes) {
+  if (!device_bytes || !pinned_bytes) return fail(VLY_ERR_INVALID, "null");
+  *device_bytes = g_held_bytes[0];
+  *pinned_bytes = g_held_bytes[1];
   return VLY_OK;
 }
 
@@ -461,6 +503,8 @@ extern "C" int vly_load_weight(vly_ctx* c, const char* name, const void* dev_ptr
   if (!c || !name || !dev_ptr || !shape || ndim < 1 || ndim > 4) return fail(VLY_ERR_INVALID, "vly_load_weight: bad argument");
   std::lock_guard<std::mutex> lk(c->mu);
   if (c->finalized) return fail(VLY_ERR_STATE, "vly_load_weight(%s): weights already finalised", name);
+  if (dtype != VLY_F32 && dtype != VLY_BF16 && dtype != VLY_F16)
+    return fail(VLY_ERR_INVALID, "vly_load_weight(%s): unknown dtype %d", name, dtype);
   CK(cudaSetDevice(c->cfg.device));
   Staged s;
   s.numel = 1;
@@ -470,34 +514,21 @@ extern "C" int vly_load_weight(vly_ctx* c, const char* name, const void* dev_ptr
   }
   const std::string nm(name);
   s.is_f32 = (ndim == 1) || ends_with(nm, "position_embedding.weight");
-  auto it = c->staged.find(nm);
-  if (it != c->staged.end()) {
-    cudaFree(it->second.dev);
-    c->staged.erase(it);
-  }
-  CK(cudaMalloc(&s.dev, (size_t)s.numel * (s.is_f32 ? 4 : 2)));
+  c->staged.erase(nm);
+  TRY(s.mem.alloc((size_t)s.numel * (s.is_f32 ? 4 : 2)));
   const int blocks = (int)std::min<long long>((s.numel + 255) / 256, 4096);
   if (s.is_f32) {
-    if (dtype == VLY_F32) convert_to_f32_bf16rounded_kernel<float><<<blocks, 256>>>((const float*)dev_ptr, (float*)s.dev, s.numel);
-    else if (dtype == VLY_BF16) convert_to_f32_bf16rounded_kernel<bf16><<<blocks, 256>>>((const bf16*)dev_ptr, (float*)s.dev, s.numel);
-    else if (dtype == VLY_F16) convert_to_f32_bf16rounded_kernel<__half><<<blocks, 256>>>((const __half*)dev_ptr, (float*)s.dev, s.numel);
-    else return fail(VLY_ERR_INVALID, "vly_load_weight(%s): unknown dtype %d", name, dtype);
+    if (dtype == VLY_F32) convert_to_f32_bf16rounded_kernel<float><<<blocks, 256>>>((const float*)dev_ptr, (float*)s.mem.p, s.numel);
+    else if (dtype == VLY_BF16) convert_to_f32_bf16rounded_kernel<bf16><<<blocks, 256>>>((const bf16*)dev_ptr, (float*)s.mem.p, s.numel);
+    else convert_to_f32_bf16rounded_kernel<__half><<<blocks, 256>>>((const __half*)dev_ptr, (float*)s.mem.p, s.numel);
   } else {
-    if (dtype == VLY_F32) convert_to_bf16_kernel<float><<<blocks, 256>>>((const float*)dev_ptr, (bf16*)s.dev, s.numel);
-    else if (dtype == VLY_BF16) CK(cudaMemcpyAsync(s.dev, dev_ptr, (size_t)s.numel * 2, cudaMemcpyDeviceToDevice, 0));
-    else if (dtype == VLY_F16) convert_to_bf16_kernel<__half><<<blocks, 256>>>((const __half*)dev_ptr, (bf16*)s.dev, s.numel);
-    else return fail(VLY_ERR_INVALID, "vly_load_weight(%s): unknown dtype %d", name, dtype);
+    if (dtype == VLY_F32) convert_to_bf16_kernel<float><<<blocks, 256>>>((const float*)dev_ptr, (bf16*)s.mem.p, s.numel);
+    else if (dtype == VLY_BF16) CK(cudaMemcpyAsync(s.mem.p, dev_ptr, (size_t)s.numel * 2, cudaMemcpyDeviceToDevice, 0));
+    else convert_to_bf16_kernel<__half><<<blocks, 256>>>((const __half*)dev_ptr, (bf16*)s.mem.p, s.numel);
   }
   CKL();
   CK(cudaStreamSynchronize(0));  // the caller may free its tensor right after we return
-  c->staged[nm] = s;
-  return VLY_OK;
-}
-
-template <typename T>
-static int dalloc(vly_ctx* c, T** p, size_t n) {
-  CK(cudaMalloc((void**)p, n * sizeof(T)));
-  c->owned.push_back(*p);
+  c->staged[nm] = std::move(s);
   return VLY_OK;
 }
 
@@ -507,16 +538,19 @@ static int get_staged(vly_ctx* c, const std::string& name, bool f32, int64_t num
   if (it->second.is_f32 != f32 || it->second.numel != numel)
     return fail(VLY_ERR_INVALID, "vly_finalize_weights: tensor '%s' has %lld elements (expected %lld)", name.c_str(),
                 (long long)it->second.numel, (long long)numel);
-  *out = it->second.dev;
+  *out = it->second.mem.p;
   return VLY_OK;
 }
-static void drop_staged(vly_ctx* c, const std::string& name) {
+// A tensor that needs no packing is staged in its final format: its staging allocation becomes the packed weight.
+static int take(vly_ctx* c, const std::string& name, bool f32, int64_t numel, Mem* dst) {
+  void* p;
+  TRY(get_staged(c, name, f32, numel, &p));
   auto it = c->staged.find(name);
-  if (it != c->staged.end()) {
-    cudaFree(it->second.dev);
-    c->staged.erase(it);
-  }
+  *dst = std::move(it->second.mem);
+  c->staged.erase(it);
+  return VLY_OK;
 }
+static void drop_staged(vly_ctx* c, const std::string& name) { c->staged.erase(name); }
 
 extern "C" int vly_finalize_weights(vly_ctx* c) {
   if (!c) return fail(VLY_ERR_INVALID, "null ctx");
@@ -533,23 +567,16 @@ extern "C" int vly_finalize_weights(vly_ctx* c) {
     const int D = g.vit_hidden, M = g.vit_mlp, P = g.vit_patch, KK = 3 * P * P;
     c->kpad = ((KK + 63) / 64) * 64;
     const int tokens = (g.vit_image / P) * (g.vit_image / P) + 1;
-    void *pw, *cls, *pos, *pg, *pb;
+    void* pw;
     TRY(get_staged(c, vp + "embeddings.patch_embedding.weight", false, (int64_t)D * KK, &pw));
-    TRY(get_staged(c, vp + "embeddings.class_embedding", true, D, &cls));
-    TRY(get_staged(c, vp + "embeddings.position_embedding.weight", true, (int64_t)tokens * D, &pos));
-    TRY(get_staged(c, vp + "pre_layrnorm.weight", true, D, &pg));
-    TRY(get_staged(c, vp + "pre_layrnorm.bias", true, D, &pb));
-    TRY(dalloc(c, &c->patch_w, (size_t)D * c->kpad));
+    TRY(take(c, vp + "embeddings.class_embedding", true, D, &c->cls));
+    TRY(take(c, vp + "embeddings.position_embedding.weight", true, (int64_t)tokens * D, &c->pos));
+    TRY(take(c, vp + "pre_layrnorm.weight", true, D, &c->pre_g));
+    TRY(take(c, vp + "pre_layrnorm.bias", true, D, &c->pre_b));
+    TRY(c->patch_w.alloc((size_t)D * c->kpad * 2));
     pack_rows_kernel<<<D, 256>>>((bf16*)pw, KK, nullptr, nullptr, nullptr, c->patch_w, c->kpad, 0, 0, nullptr, nullptr);
     CKL();
-    TRY(dalloc(c, &c->cls, D));
-    TRY(dalloc(c, &c->pos, (size_t)tokens * D));
-    TRY(dalloc(c, &c->pre_g, D));
-    TRY(dalloc(c, &c->pre_b, D));
-    CK(cudaMemcpy(c->cls, cls, D * 4, cudaMemcpyDeviceToDevice));
-    CK(cudaMemcpy(c->pos, pos, (size_t)tokens * D * 4, cudaMemcpyDeviceToDevice));
-    CK(cudaMemcpy(c->pre_g, pg, D * 4, cudaMemcpyDeviceToDevice));
-    CK(cudaMemcpy(c->pre_b, pb, D * 4, cudaMemcpyDeviceToDevice));
+    CK(cudaDeviceSynchronize());
     drop_staged(c, vp + "embeddings.patch_embedding.weight");
     c->vit.resize(g.vit_layers);
     for (int l = 0; l < g.vit_layers; ++l) {
@@ -560,9 +587,9 @@ extern "C" int vly_finalize_weights(vly_ctx* c) {
       TRY(get_staged(c, q + "layer_norm1.bias", true, D, &b1n));
       TRY(get_staged(c, q + "layer_norm2.weight", true, D, &g2));
       TRY(get_staged(c, q + "layer_norm2.bias", true, D, &b2n));
-      TRY(dalloc(c, &w.wqkv, (size_t)3 * D * D));
-      TRY(dalloc(c, &w.qkv_cs, 3 * D));
-      TRY(dalloc(c, &w.qkv_b, 3 * D));
+      TRY(w.wqkv.alloc((size_t)3 * D * D * 2));
+      TRY(w.qkv_cs.alloc(3 * D * 4));
+      TRY(w.qkv_b.alloc(3 * D * 4));
       const char* nm[3] = {"q_proj", "k_proj", "v_proj"};
       for (int i = 0; i < 3; ++i) {
         void *ww, *bb;
@@ -573,45 +600,29 @@ extern "C" int vly_finalize_weights(vly_ctx* c) {
         CK(cudaDeviceSynchronize());
         drop_staged(c, q + "self_attn." + nm[i] + ".weight");
       }
-      void *wo, *bo, *w1, *b1, *w2, *b2;
-      TRY(get_staged(c, q + "self_attn.out_proj.weight", false, (int64_t)D * D, &wo));
-      TRY(get_staged(c, q + "self_attn.out_proj.bias", true, D, &bo));
+      void *w1, *b1;
+      TRY(take(c, q + "self_attn.out_proj.weight", false, (int64_t)D * D, &w.wo));
+      TRY(take(c, q + "self_attn.out_proj.bias", true, D, &w.bo));
       TRY(get_staged(c, q + "mlp.fc1.weight", false, (int64_t)M * D, &w1));
       TRY(get_staged(c, q + "mlp.fc1.bias", true, M, &b1));
-      TRY(get_staged(c, q + "mlp.fc2.weight", false, (int64_t)D * M, &w2));
-      TRY(get_staged(c, q + "mlp.fc2.bias", true, D, &b2));
-      TRY(dalloc(c, &w.wo, (size_t)D * D));
-      TRY(dalloc(c, &w.bo, D));
-      TRY(dalloc(c, &w.w1, (size_t)M * D));
-      TRY(dalloc(c, &w.c1, M));
-      TRY(dalloc(c, &w.b1, M));
-      TRY(dalloc(c, &w.w2, (size_t)D * M));
-      TRY(dalloc(c, &w.b2, D));
-      CK(cudaMemcpy(w.wo, wo, (size_t)D * D * 2, cudaMemcpyDeviceToDevice));
-      CK(cudaMemcpy(w.bo, bo, D * 4, cudaMemcpyDeviceToDevice));
+      TRY(take(c, q + "mlp.fc2.weight", false, (int64_t)D * M, &w.w2));
+      TRY(take(c, q + "mlp.fc2.bias", true, D, &w.b2));
+      TRY(w.w1.alloc((size_t)M * D * 2));
+      TRY(w.c1.alloc(M * 4));
+      TRY(w.b1.alloc(M * 4));
       pack_rows_kernel<<<M, 256>>>((bf16*)w1, D, (float*)g2, (float*)b2n, (float*)b1, w.w1, D, 0, 0, w.c1, w.b1);
       CKL();
-      CK(cudaMemcpy(w.w2, w2, (size_t)D * M * 2, cudaMemcpyDeviceToDevice));
-      CK(cudaMemcpy(w.b2, b2, D * 4, cudaMemcpyDeviceToDevice));
       CK(cudaDeviceSynchronize());
-      drop_staged(c, q + "self_attn.out_proj.weight");
       drop_staged(c, q + "mlp.fc1.weight");
-      drop_staged(c, q + "mlp.fc2.weight");
     }
     if (c->staged.count("model.mm_projector.weight")) {
-      void *pjw, *pjb;
-      TRY(get_staged(c, "model.mm_projector.weight", false, (int64_t)g.hidden_size * D, &pjw));
-      TRY(get_staged(c, "model.mm_projector.bias", true, g.hidden_size, &pjb));
-      TRY(dalloc(c, &c->proj_w, (size_t)g.hidden_size * D));
-      TRY(dalloc(c, &c->proj_b, g.hidden_size));
-      CK(cudaMemcpy(c->proj_w, pjw, (size_t)g.hidden_size * D * 2, cudaMemcpyDeviceToDevice));
-      CK(cudaMemcpy(c->proj_b, pjb, g.hidden_size * 4, cudaMemcpyDeviceToDevice));
-      drop_staged(c, "model.mm_projector.weight");
+      TRY(take(c, "model.mm_projector.weight", false, (int64_t)g.hidden_size * D, &c->proj_w));
+      TRY(take(c, "model.mm_projector.bias", true, g.hidden_size, &c->proj_b));
       const int H = g.hidden_size, NP = (g.vit_image / g.vit_patch) * (g.vit_image / g.vit_patch);
       if (g.patch_pooling_method == VLY_POOL_TEMPORAL_IMPORTANCE) {       // valley_model.py:40-43
         void* pw;
         TRY(get_staged(c, "model.pooling_layer.weight", false, (int64_t)NP * H, &pw));
-        TRY(dalloc(c, &c->pool_U, (size_t)NP * D));
+        TRY(c->pool_U.alloc((size_t)NP * D * 4));
         fold_importance_kernel<<<NP, 256>>>((const bf16*)pw, c->proj_w, c->pool_U, H, D);      // the bias cancels in the softmax
         CKL();
         CK(cudaDeviceSynchronize());
@@ -625,38 +636,22 @@ extern "C" int vly_finalize_weights(vly_ctx* c) {
         auto ip = c->staged.find("model.position_matrix");
         if (ip == c->staged.end()) return fail(VLY_ERR_STATE, "vly_finalize_weights: missing tensor 'model.position_matrix'");
         w.max_pos = (int)(ip->second.numel / H);
-        struct { const char* name; bool f32; int64_t n; void** dst; } items[] = {
-            {"self_attn.in_proj_weight", false, (int64_t)3 * H * H, (void**)&w.in_w}, {"self_attn.in_proj_bias", true, 3 * H, (void**)&w.in_b},
-            {"self_attn.out_proj.weight", false, (int64_t)H * H, (void**)&w.out_w},   {"self_attn.out_proj.bias", true, H, (void**)&w.out_b},
-            {"linear1.weight", false, (int64_t)w.ffn * H, (void**)&w.l1_w},           {"linear1.bias", true, w.ffn, (void**)&w.l1_b},
-            {"linear2.weight", false, (int64_t)H * w.ffn, (void**)&w.l2_w},           {"linear2.bias", true, H, (void**)&w.l2_b},
-            {"norm1.weight", true, H, (void**)&w.n1_g}, {"norm1.bias", true, H, (void**)&w.n1_b},
-            {"norm2.weight", true, H, (void**)&w.n2_g}, {"norm2.bias", true, H, (void**)&w.n2_b}};
-        for (auto& it2 : items) {
-          void* src;
-          TRY(get_staged(c, q + it2.name, it2.f32, it2.n, &src));
-          const size_t bytes = (size_t)it2.n * (it2.f32 ? 4 : 2);
-          CK(cudaMalloc(it2.dst, bytes));
-          c->owned.push_back(*it2.dst);
-          CK(cudaMemcpy(*it2.dst, src, bytes, cudaMemcpyDeviceToDevice));
-          drop_staged(c, q + it2.name);
-        }
-        void* pm;
-        TRY(get_staged(c, "model.position_matrix", false, (int64_t)w.max_pos * H, &pm));
-        TRY(dalloc(c, &w.pos, (size_t)w.max_pos * H));
-        CK(cudaMemcpy(w.pos, pm, (size_t)w.max_pos * H * 2, cudaMemcpyDeviceToDevice));
-        drop_staged(c, "model.position_matrix");
+        struct { const char* name; bool f32; int64_t n; Mem* dst; } items[] = {
+            {"self_attn.in_proj_weight", false, (int64_t)3 * H * H, &w.in_w}, {"self_attn.in_proj_bias", true, 3 * H, &w.in_b},
+            {"self_attn.out_proj.weight", false, (int64_t)H * H, &w.out_w},   {"self_attn.out_proj.bias", true, H, &w.out_b},
+            {"linear1.weight", false, (int64_t)w.ffn * H, &w.l1_w},           {"linear1.bias", true, w.ffn, &w.l1_b},
+            {"linear2.weight", false, (int64_t)H * w.ffn, &w.l2_w},           {"linear2.bias", true, H, &w.l2_b},
+            {"norm1.weight", true, H, &w.n1_g}, {"norm1.bias", true, H, &w.n1_b},
+            {"norm2.weight", true, H, &w.n2_g}, {"norm2.bias", true, H, &w.n2_b}};
+        for (auto& it2 : items) TRY(take(c, q + it2.name, it2.f32, it2.n, it2.dst));
+        TRY(take(c, "model.position_matrix", false, (int64_t)w.max_pos * H, &w.pos));
       }
     }
   }
 
   if (c->has_llm) {
     const int H = g.hidden_size, I = g.intermediate_size, V = g.vocab_size, L = g.num_hidden_layers;
-    void* emb;
-    TRY(get_staged(c, "model.embed_tokens.weight", false, (int64_t)V * H, &emb));
-    TRY(dalloc(c, &c->embed, (size_t)V * H));
-    CK(cudaMemcpy(c->embed, emb, (size_t)V * H * 2, cudaMemcpyDeviceToDevice));
-    drop_staged(c, "model.embed_tokens.weight");
+    TRY(take(c, "model.embed_tokens.weight", false, (int64_t)V * H, &c->embed));
     c->layers.resize(L);
     for (int l = 0; l < L; ++l) {
       const std::string q = "model.layers." + std::to_string(l) + ".";
@@ -664,7 +659,7 @@ extern "C" int vly_finalize_weights(vly_ctx* c) {
       void *g1, *g2;
       TRY(get_staged(c, q + "input_layernorm.weight", true, H, &g1));
       TRY(get_staged(c, q + "post_attention_layernorm.weight", true, H, &g2));
-      TRY(dalloc(c, &w.wqkv, (size_t)3 * H * H));
+      TRY(w.wqkv.alloc((size_t)3 * H * H * 2));
       const char* nm[3] = {"q_proj", "k_proj", "v_proj"};
       for (int i = 0; i < 3; ++i) {
         void* ww;
@@ -674,39 +669,32 @@ extern "C" int vly_finalize_weights(vly_ctx* c) {
         CK(cudaDeviceSynchronize());
         drop_staged(c, q + "self_attn." + nm[i] + ".weight");
       }
-      void *wo, *wg, *wu, *wd;
-      TRY(get_staged(c, q + "self_attn.o_proj.weight", false, (int64_t)H * H, &wo));
+      void *wg, *wu;
+      TRY(take(c, q + "self_attn.o_proj.weight", false, (int64_t)H * H, &w.wo));
       TRY(get_staged(c, q + "mlp.gate_proj.weight", false, (int64_t)I * H, &wg));
       TRY(get_staged(c, q + "mlp.up_proj.weight", false, (int64_t)I * H, &wu));
-      TRY(get_staged(c, q + "mlp.down_proj.weight", false, (int64_t)H * I, &wd));
-      TRY(dalloc(c, &w.wo, (size_t)H * H));
-      TRY(dalloc(c, &w.wgu, (size_t)2 * I * H));
-      TRY(dalloc(c, &w.wdown, (size_t)H * I));
-      CK(cudaMemcpy(w.wo, wo, (size_t)H * H * 2, cudaMemcpyDeviceToDevice));
+      TRY(take(c, q + "mlp.down_proj.weight", false, (int64_t)H * I, &w.wdown));
+      TRY(w.wgu.alloc((size_t)2 * I * H * 2));
       pack_rows_kernel<<<I, 256>>>((bf16*)wg, H, (float*)g2, nullptr, nullptr, w.wgu, H, 2, 0, nullptr, nullptr);
       pack_rows_kernel<<<I, 256>>>((bf16*)wu, H, (float*)g2, nullptr, nullptr, w.wgu, H, 2, 1, nullptr, nullptr);
       CKL();
-      CK(cudaMemcpy(w.wdown, wd, (size_t)H * I * 2, cudaMemcpyDeviceToDevice));
       CK(cudaDeviceSynchronize());
-      drop_staged(c, q + "self_attn.o_proj.weight");
       drop_staged(c, q + "mlp.gate_proj.weight");
       drop_staged(c, q + "mlp.up_proj.weight");
-      drop_staged(c, q + "mlp.down_proj.weight");
     }
     void *nf, *lm;
     TRY(get_staged(c, "model.norm.weight", true, H, &nf));
     TRY(get_staged(c, "lm_head.weight", false, (int64_t)V * H, &lm));
-    TRY(dalloc(c, &c->lm_head, (size_t)V * H));
+    TRY(c->lm_head.alloc((size_t)V * H * 2));
     pack_rows_kernel<<<V, 256>>>((bf16*)lm, H, (float*)nf, nullptr, nullptr, c->lm_head, H, 0, 0, nullptr, nullptr);
     CKL();
     CK(cudaDeviceSynchronize());
     drop_staged(c, "lm_head.weight");
-    TRY(dalloc(c, &c->rope, (size_t)g.max_position_embeddings * 64));
+    TRY(c->rope.alloc((size_t)g.max_position_embeddings * 64 * sizeof(float2)));
     rope_table_kernel<<<cdiv((long long)g.max_position_embeddings * 64, 256), 256>>>(c->rope, g.max_position_embeddings, g.rope_theta, 128);
     CKL();
   }
   CK(cudaDeviceSynchronize());
-  for (auto& kvp : c->staged) cudaFree(kvp.second.dev);
   c->staged.clear();
   c->finalized = true;
   return VLY_OK;
@@ -864,7 +852,7 @@ __global__ void gather_wait_kernel(volatile int* flags, int world, int epoch, in
 // timeout flag.  The gather buffer then holds partially written or previous-epoch rows, so every later gather call -- and
 // vly_gather_status, which callers poll after their next synchronisation -- fails loudly instead of decoding stale features.
 static int gather_check_timeout(vly_ctx* c, const char* who) {
-  if (c->g_timeout && *reinterpret_cast<volatile int*>(c->g_timeout) != 0)
+  if (c->g_timeout && *reinterpret_cast<volatile int*>(c->g_timeout.p) != 0)
     return fail(VLY_ERR_STATE, "%s: a peer rank never signalled its frame features (fused all-gather timed out); the gather "
                 "buffer is stale -- the process group must be torn down", who);
   return VLY_OK;
@@ -872,7 +860,7 @@ static int gather_check_timeout(vly_ctx* c, const char* who) {
 
 extern "C" int vly_gather_status(vly_ctx* c, int* timed_out) {
   if (!c || !timed_out) return fail(VLY_ERR_INVALID, "vly_gather_status: null argument");
-  *timed_out = (c->g_timeout && *reinterpret_cast<volatile int*>(c->g_timeout) != 0) ? 1 : 0;
+  *timed_out = (c->g_timeout && *reinterpret_cast<volatile int*>(c->g_timeout.p) != 0) ? 1 : 0;
   return *timed_out ? gather_check_timeout(c, "vly_gather_status") : VLY_OK;
 }
 
@@ -882,21 +870,21 @@ extern "C" int vly_gather_create(vly_ctx* c, int64_t rows_total, void** local_bu
   CK(cudaSetDevice(c->cfg.device));
   if (c->g_buf) return fail(VLY_ERR_STATE, "vly_gather_create: a gather buffer already exists for this context");
   const size_t data = (((size_t)rows_total * c->cfg.vit_hidden * 2) + 255) & ~size_t(255);
-  void* base;
-  CK(cudaMalloc(&base, data + 256));
-  CK(cudaMemset(base, 0, data + 256));
-  c->g_buf = (bf16*)base;
-  c->g_rows = rows_total;
-  c->g_flags = (int*)((char*)base + data);
+  Owned<bf16> buf;
+  TRY(buf.alloc(data + 256));
+  CK(cudaMemset(buf, 0, data + 256));
   if (!c->g_timeout) {
-    CK(cudaHostAlloc((void**)&c->g_timeout, sizeof(int), cudaHostAllocMapped));
+    TRY(c->g_timeout.alloc(sizeof(int), true));
     *c->g_timeout = 0;
   }
   cudaIpcMemHandle_t h;
-  CK(cudaIpcGetMemHandle(&h, base));
+  CK(cudaIpcGetMemHandle(&h, buf));
   static_assert(sizeof(cudaIpcMemHandle_t) == 64, "CUDA IPC handle size");
   memcpy(handle_out, &h, 64);
-  *local_buf = base;
+  *local_buf = buf;
+  c->g_buf = std::move(buf);
+  c->g_rows = rows_total;
+  c->g_flags = (int*)((char*)c->g_buf.p + data);
   return VLY_OK;
 }
 
@@ -1252,9 +1240,9 @@ static int plan_decode_mega(vly_ctx* c, vly_kv* kv, const DecodeSettings& s) {
     for (int i = 0; i < 5 && i < (int)ph.size(); ++i)
       if (ph[i].type != PH_ATTN) fprintf(stderr, " type%d N=%d K=%d rows=%d kc=%d inflight=%d;", ph[i].type, ph[i].N, ph[i].K, ph[i].rows, ph[i].kc, ph[i].inflight);
     fprintf(stderr, " logits rows=%d kc=%d\n", ph.back().rows, ph.back().kc);
-    CK(cudaMalloc((void**)&kv->dbg, kMegaDbgCounters * sizeof(long long)));
+    TRY(kv->dbg.alloc(kMegaDbgCounters * sizeof(long long)));
   }
-  CK(cudaMalloc((void**)&kv->d_phases, ph.size() * sizeof(PhaseDesc)));
+  TRY(kv->d_phases.alloc(ph.size() * sizeof(PhaseDesc)));
   CK(cudaMemcpy(kv->d_phases, ph.data(), ph.size() * sizeof(PhaseDesc), cudaMemcpyHostToDevice));
 
   StepParams& p = kv->mega;
@@ -1290,55 +1278,49 @@ extern "C" int vly_kv_create(vly_ctx* c, int batch, int max_seq, vly_kv** out) {
   if (max_seq > c->cfg.max_position_embeddings) return fail(VLY_ERR_INVALID, "vly_kv_create: max_seq %d > max_position_embeddings %d", max_seq, c->cfg.max_position_embeddings);
   CK(cudaSetDevice(c->cfg.device));
   const vly_config& g = c->cfg;
-  vly_kv* kv = new vly_kv();
+  auto kv = std::make_unique<vly_kv>();
   kv->ctx = c;
   kv->B = batch;
   kv->Smax = (max_seq + 127) / 128 * 128;   // whole 128-key TMA tiles
   const int H = g.hidden_size, nH = g.num_attention_heads, I = g.intermediate_size, V = g.vocab_size, L = g.num_hidden_layers;
   const size_t cache_elems = (size_t)L * kv->layer_stride();
-  CK(cudaMalloc((void**)&kv->cache, cache_elems * 2));
+  TRY(kv->cache.alloc(cache_elems * 2));
   CK(cudaMemset(kv->cache, 0, cache_elems * 2));   // padded keys must be finite: P(=0) * V(pad) must stay 0
   kv->nsplit = kv->Smax / MegaCfg::ATTN_KEYS_MIN;   // capacity of the split dimension: the persistent kernel uses 16/32-key items,
                                                     // the per-op kernel fixed 64-key splits (it only touches the first Smax / 64 slots)
-  CK(cudaMalloc((void**)&kv->d_len, 8));
-  CK(cudaHostAlloc((void**)&kv->h_len, sizeof(int), cudaHostAllocDefault));
+  TRY(kv->d_len.alloc(8));
+  TRY(kv->h_len.alloc(sizeof(int), true));
   CK(cudaEventCreateWithFlags(&kv->len_event, cudaEventDisableTiming));
   kv->d_step = kv->d_len + 1;
   CK(cudaMemset(kv->d_len, 0, 8));
   // (at least 8 rows, rows >= batch stay zero)
   const size_t act_rows = batch < 8 ? 8 : batch;
-  CK(cudaMalloc((void**)&kv->x, act_rows * H * 2));
-  CK(cudaMalloc((void**)&kv->q, act_rows * H * 2));
-  CK(cudaMalloc((void**)&kv->attn, act_rows * H * 2));
-  CK(cudaMalloc((void**)&kv->hb, act_rows * I * 2));
+  TRY(kv->x.alloc(act_rows * H * 2));
+  TRY(kv->q.alloc(act_rows * H * 2));
+  TRY(kv->attn.alloc(act_rows * H * 2));
+  TRY(kv->hb.alloc(act_rows * I * 2));
   CK(cudaMemset(kv->x, 0, act_rows * H * 2));
   CK(cudaMemset(kv->attn, 0, act_rows * H * 2));
   CK(cudaMemset(kv->hb, 0, act_rows * I * 2));
-  CK(cudaMalloc((void**)&kv->part_o, (size_t)batch * nH * kv->nsplit * 128 * 4));
-  CK(cudaMalloc((void**)&kv->part_ml, (size_t)batch * nH * kv->nsplit * sizeof(float2)));
-  CK(cudaMalloc((void**)&kv->counters, ((size_t)batch * nH + 4) * 4));
+  TRY(kv->part_o.alloc((size_t)batch * nH * kv->nsplit * 128 * 4));
+  TRY(kv->part_ml.alloc((size_t)batch * nH * kv->nsplit * sizeof(float2)));
+  TRY(kv->counters.alloc(((size_t)batch * nH + 4) * 4));
   CK(cudaMemset(kv->counters, 0, ((size_t)batch * nH + 4) * 4));
-  CK(cudaMalloc((void**)&kv->part_val, (size_t)batch * c->num_sms * 4));   // every arg-max kernel runs at most one CTA per SM
-  CK(cudaMalloc((void**)&kv->part_idx, (size_t)batch * c->num_sms * 4));
-  CK(cudaMalloc((void**)&kv->logits, (size_t)batch * V * 4));
-  CK(cudaMalloc((void**)&kv->cur_tokens, (size_t)batch * 8));
-  CK(cudaMalloc((void**)&kv->gen_tokens, (size_t)batch * kv->Smax * 8));
-  CK(cudaMalloc((void**)&kv->d_sample, sizeof(SampleState)));
+  TRY(kv->part_val.alloc((size_t)batch * c->num_sms * 4));   // every arg-max kernel runs at most one CTA per SM
+  TRY(kv->part_idx.alloc((size_t)batch * c->num_sms * 4));
+  TRY(kv->logits.alloc((size_t)batch * V * 4));
+  TRY(kv->cur_tokens.alloc((size_t)batch * 8));
+  TRY(kv->gen_tokens.alloc((size_t)batch * kv->Smax * 8));
+  TRY(kv->d_sample.alloc(sizeof(SampleState)));
   {
     SampleState s0 = {};
     s0.inv_temp = 1.f; s0.eos = -1; s0.pad = 0; s0.stop2 = -1;
     CK(cudaMemcpy(kv->d_sample, &s0, sizeof(s0), cudaMemcpyHostToDevice));
   }
-  CK(cudaMalloc((void**)&kv->key_bits, (size_t)batch * kv->mask_words() * 4));
+  TRY(kv->key_bits.alloc((size_t)batch * kv->mask_words() * 4));
   CK(cudaMemset(kv->key_bits, 0xff, (size_t)batch * kv->mask_words() * 4));
-  if (batch <= 4) {
-    const int r = plan_decode_mega(c, kv, read_decode_settings());
-    if (r != VLY_OK) {
-      vly_kv_destroy(kv);
-      return r;
-    }
-  }
-  *out = kv;
+  if (batch <= 4) TRY(plan_decode_mega(c, kv.get(), read_decode_settings()));
+  *out = kv.release();
   return VLY_OK;
 }
 
@@ -1353,13 +1335,6 @@ extern "C" int vly_kv_decode_kernel(vly_kv* kv, char* name, int cap) {
 extern "C" void vly_kv_destroy(vly_kv* kv) {
   if (!kv) return;
   cudaSetDevice(kv->ctx->cfg.device);
-  if (kv->graph) cudaGraphExecDestroy(kv->graph);
-  if (kv->graph_n) cudaGraphExecDestroy(kv->graph_n);
-  if (kv->h_len) cudaFreeHost(kv->h_len);
-  if (kv->len_event) cudaEventDestroy(kv->len_event);
-  void* ps[] = {kv->d_sample, kv->key_bits, kv->dbg, kv->d_phases, kv->cache, kv->d_len, kv->x, kv->q, kv->attn, kv->hb, kv->part_o, kv->part_ml, kv->counters, kv->part_val, kv->part_idx, kv->logits, kv->cur_tokens, kv->gen_tokens};
-  for (void* p : ps)
-    if (p) cudaFree(p);
   delete kv;
 }
 
@@ -1544,7 +1519,7 @@ static int launch_prefill_attention(vly_ctx* c, vly_kv* kv, const bf16* qbuf, in
   PrefillAttnParams p;
   p.B = B; p.S = S; p.past = past; p.nH = nH; p.H = H; p.Smax = kv->Smax; p.ctx = out;
   p.scale_log2e = 0.08838834764831845f * 1.4426950408889634f;
-  p.key_bits = kv->masked ? kv->key_bits : nullptr; p.mask_words = kv->mask_words();
+  p.key_bits = kv->masked ? static_cast<uint32_t*>(kv->key_bits) : nullptr; p.mask_words = kv->mask_words();
   const int n_qt = cdiv(S, 64);
   CK(launch_ex(llama_prefill_attention_kernel, dim3(B * nH * n_qt), dim3(C::THREADS), C::SMEM_BYTES, st, true, tq, tk, tv, p));
   c->launches++;

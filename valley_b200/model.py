@@ -172,14 +172,18 @@ class ValleyKVCache:
         m = (attention_mask != 0).to(self._model.device, torch.uint8).contiguous()
         check(self._model._lib.vly_kv_set_key_mask(self._h, m.data_ptr(), total_len, _stream()))
 
+    def release(self):
+        """Give the handle (allocation + captured CUDA graphs) back to the model for the next cache of the same shape, or
+        destroy it when the model already keeps 2.  The cache is unusable afterwards."""
+        h, self._h = getattr(self, "_h", None), None
+        if h is not None and self._model._ctx and not self._model._push_handle(self.batch, self.max_seq, h):
+            self._model._lib.vly_kv_destroy(h)
+
     def __del__(self):
         # forward() without past_key_values hands a fresh cache to the caller on every request (model_worker.py:371-379);
         # when the caller drops it, the allocation (1 GB / sequence at 7B) goes back to the model instead of to cudaFree
         try:
-            if getattr(self, "_h", None) is not None and self._model._ctx:
-                if not self._model._push_handle(self.batch, self.max_seq, self._h):
-                    self._model._lib.vly_kv_destroy(self._h)
-                self._h = None
+            self.release()
         except Exception:
             pass
 
@@ -356,8 +360,8 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
         self.training = False
         self.logits_all_positions = True      # reference behaviour (valley_model.py:304-305); generate() uses last-only
         import threading
-        self._cache_pool, self._pool_lock = {}, threading.Lock()
-        self._free_handles = {}               # (batch, max_seq) -> [vly_kv handles] released by dropped ValleyKVCache objects
+        self._pool_lock = threading.Lock()
+        self._free_handles = {}               # (batch, max_seq) -> [vly_kv handles] released by ValleyKVCache.release()
 
     # ---------------- lifetime / weights ----------------
     def __del__(self):
@@ -584,23 +588,13 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
         return ValleyKVCache(self, batch, max_seq or self.config.max_position_embeddings)
 
     def _borrow_cache(self, batch: int) -> ValleyKVCache:
-        """generate() recycles its KV caches (and the CUDA graph captured on them) instead of paying a
-        multi-GB cudaMalloc + graph capture per request.  The pool is per model instance and lock-protected
-        (model_worker.py:467-474 calls the model from several threads)."""
-        with self._pool_lock:
-            lst = self._cache_pool.setdefault(batch, [])
-            c = lst.pop() if lst else None
-        if c is None:
-            c = self.new_cache(batch)
-        else:
-            c.reset()
-        return c
+        """generate() recycles its KV-cache handles (and the CUDA graphs captured on them) through the model's handle pool
+        instead of paying a multi-GB cudaMalloc + graph capture per request.  The pool is per model instance and
+        lock-protected (model_worker.py:467-474 calls the model from several threads)."""
+        return self.new_cache(batch)
 
     def _return_cache(self, c: ValleyKVCache):
-        with self._pool_lock:
-            lst = self._cache_pool.setdefault(c.batch, [])
-            if len(lst) < 2:
-                lst.append(c)
+        c.release()
 
     def _prefill(self, cache: ValleyKVCache, embeds: torch.Tensor, logits_mode: int):
         B, S, _ = embeds.shape
