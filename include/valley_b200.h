@@ -189,13 +189,21 @@ int vly_cross_entropy(vly_ctx* ctx, const float* logits_dev, const int64_t* labe
  * temperature < 1e-4: arg-max (model_worker.py:390-391); otherwise multinomial(softmax(logits / temperature)) (:392-395), drawn
  * with the Gumbel-max identity from counter-based Philox noise keyed by `seed` -- fused into the arg-max epilogue of the decode
  * step, so sampling costs no extra pass and no host round trip.  eos_token_id >= 0: a row that emits it is finished (:396-397);
- * finished rows emit pad_token_id (HF generate) and once every row has finished the remaining steps are skipped. */
+ * finished rows emit pad_token_id (HF generate) and once every row has finished the remaining steps are skipped.
+ * top_k / top_p (HF generate's TopKLogitsWarper / TopPLogitsWarper, applied after the temperature and only when sampling):
+ * with s = logits / temperature, top_k keeps the tokens whose s is >= the k-th largest s (ties kept; k >= V keeps all);
+ * top_p then keeps, among those, every token whose score has less than top_p of the softmax mass strictly above it (the
+ * maximum is always kept; a tie group at the cut is kept whole).  The token is the same Gumbel-max draw restricted to the kept
+ * set, so a filter that keeps everything draws what the unfiltered sampler draws.  With a filter on, one more kernel per step
+ * (one CTA per row over the step's logits) makes the selection.  Zero-initialised fields mean no filter. */
 typedef struct {
   float temperature;
   uint64_t seed;
   int64_t eos_token_id;      /* -1: none */
   int64_t pad_token_id;
   int64_t stop_token_id;     /* -1: none; a second id that ends a row: the worker's single-token stop string (model_worker.py:355-360, :396-397) */
+  int32_t top_k;             /* <= 0: off */
+  float top_p;               /* off unless 0 < top_p < 1 */
 } vly_sampling;
 
 /* the first generated token: select from the prefill's last-position logits [B,V] fp32 (vly_llama_prefill logits_mode 1);
@@ -228,6 +236,10 @@ int vly_test_gemm(vly_ctx* ctx, const void* a_dev, const void* w_dev, int M, int
                   const void* residual_dev, void* out_dev, int block_n, void* stream);
 /* ViT attention on a packed qkv [F*257, 3072] bf16 -> ctx [F*257,1024] bf16 */
 int vly_test_vit_attention(vly_ctx* ctx, const void* qkv_dev, int n_frames, void* out_dev, void* stream);
+/* the top-k / top-p filter of vly_sampling over logits [B,V] fp32 (any V): keep_out [B,V] uint8 = 1 where the token is kept,
+ * computed by the same device routine the decode loop selects with.  temperature > 0; top_k / top_p as in vly_sampling. */
+int vly_test_sample_filter(vly_ctx* ctx, const float* logits_dev, int B, int V, float temperature, int top_k, float top_p,
+                           uint8_t* keep_out_dev, void* stream);
 
 #ifdef __cplusplus
 }

@@ -4,13 +4,16 @@
 one process (the weights are loaded once).  The library reads them when a KV cache is created and the cache keeps them, so
 every configuration gets a KV cache of its own, created with its variables set, and the configurations are timed
 round-robin for --rounds rounds.  '' (an empty configuration) is the library's defaults.  With VLY_MEGA_DBG=1 each
-configuration's cycle counters are read from its own cache."""
+configuration's cycle counters are read from its own cache.
+
+--sampling 'greedy;0.7;0.7,50;0.7,50,0.9' times token selection settings the same way: 'greedy', or 'T[,top_k[,top_p]]'
+(temperature sampling, with HF generate's top-k / top-p filters).  Every configuration is timed with every setting."""
 import argparse, os, statistics, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import torch
 from valley_b200 import synthetic as syn
-from valley_b200._lib import check
+from valley_b200._lib import VlySampling, check
 from valley_b200.model import ValleyConfig, ValleyLlamaForCausalLM
 
 ap = argparse.ArgumentParser()
@@ -19,6 +22,7 @@ ap.add_argument("--batch", type=int, default=1)
 ap.add_argument("--steps", type=int, default=120)
 ap.add_argument("--configs", default=None, help="';'-separated list of 'VAR=value,VAR=value' environment settings")
 ap.add_argument("--rounds", type=int, default=3)
+ap.add_argument("--sampling", default=None, help="';'-separated list of 'greedy' or 'T[,top_k[,top_p]]'")
 a = ap.parse_args()
 spec = syn.SPECS[a.model]
 m = ValleyLlamaForCausalLM(ValleyConfig.from_spec(spec), 0)
@@ -44,12 +48,24 @@ def parse(cfg):
     return env
 
 
-configs = [""] if a.configs is None else a.configs.split(";")
+def parse_sampling(text):
+    """'greedy' -> None; 'T[,top_k[,top_p]]' -> VlySampling (fixed seed, no stop token)"""
+    if text.strip() == "greedy":
+        return None
+    f = text.split(",")
+    return VlySampling(float(f[0]), 1234, -1, 0, -1, int(f[1]) if len(f) > 1 else 0, float(f[2]) if len(f) > 2 else 1.0)
+
+
+configs = [(c, s) for c in ([""] if a.configs is None else a.configs.split(";"))
+           for s in (["greedy"] if a.sampling is None else a.sampling.split(";"))]
 base_env = dict(os.environ)
 
 
-def run_config(ci, cfg):
+def run_config(ci, cfg_samp):
     """one timed run of configuration ci: fresh prefill, 8 warm-up steps, a.steps timed steps (ms per step)"""
+    import ctypes as C
+    cfg, samp = cfg_samp
+    sp = parse_sampling(samp)
     os.environ.clear()
     os.environ.update(base_env)
     os.environ.update(parse(cfg))
@@ -58,7 +74,10 @@ def run_config(ci, cfg):
     cache = m.new_cache(a.batch, ids.shape[1] + a.steps + 160 + 128 * ci)
     _, nxt = m._prefill(cache, emb, 0)
     out = torch.empty(a.batch, a.steps, dtype=torch.int64, device="cuda")
-    run = lambda n: check(m._lib.vly_generate_greedy(m._ctx, cache._h, nxt.data_ptr(), n, out.data_ptr(), 0))
+    if sp is None:
+        run = lambda n: check(m._lib.vly_generate_greedy(m._ctx, cache._h, nxt.data_ptr(), n, out.data_ptr(), 0))
+    else:
+        run = lambda n: check(m._lib.vly_generate(m._ctx, cache._h, nxt.data_ptr(), n, out.data_ptr(), C.byref(sp), None, 0))
     run(8)
     torch.cuda.synchronize()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -105,11 +124,11 @@ for rnd in range(a.rounds):
             res[ci] = (res[ci], S, toks, arr)
 os.environ.clear()
 os.environ.update(base_env)
-for ci, cfg in enumerate(configs):
+for ci, (cfg, samp) in enumerate(configs):
     times, S, toks, arr = res[ci]
     med = statistics.median(times)
     bytes_step = 2 * (L * (4 * H * H + 3 * H * I) + V * H) + a.batch * (S - a.steps // 2) * 2 * L * H * 2
-    print(f"{a.model} B={a.batch} [{cfg or 'defaults'}]: median {med:.3f} ms/token  (min {min(times):.3f}, max {max(times):.3f}, "
+    print(f"{a.model} B={a.batch} [{cfg or 'defaults'}] [{samp}]: median {med:.3f} ms/token  (min {min(times):.3f}, max {max(times):.3f}, "
           f"{len(times)} runs)  {a.batch / med * 1e3:.1f} tok/s  {bytes_step / med / 1e6:.0f} GB/s  tokens[0,:6]={toks}  "
           f"lib={os.environ.get('VLY_LIB_PATH', 'default')}")
     if arr is not None:

@@ -35,10 +35,10 @@ class VlyTokens(C.Structure):
 
 class VlySampling(C.Structure):
     _fields_ = [("temperature", C.c_float), ("seed", C.c_uint64), ("eos_token_id", C.c_int64), ("pad_token_id", C.c_int64),
-                ("stop_token_id", C.c_int64)]
+                ("stop_token_id", C.c_int64), ("top_k", C.c_int32), ("top_p", C.c_float)]
 
-    def __init__(self, temperature=0.0, seed=0, eos_token_id=-1, pad_token_id=0, stop_token_id=-1):
-        super().__init__(temperature, seed, eos_token_id, pad_token_id, stop_token_id)
+    def __init__(self, temperature=0.0, seed=0, eos_token_id=-1, pad_token_id=0, stop_token_id=-1, top_k=0, top_p=1.0):
+        super().__init__(temperature, seed, eos_token_id, pad_token_id, stop_token_id, top_k, top_p)
 
 
 VLY_OK, VLY_ERR_INVALID, VLY_ERR_CUDA, VLY_ERR_STATE = 0, -1, -2, -3
@@ -89,6 +89,7 @@ SIGNATURES = {
     "vly_set_error_": (None, [C.c_char_p]),
     "vly_test_gemm": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp]),
     "vly_test_vit_attention": (_i, [_vp, _vp, _i, _vp, _vp]),
+    "vly_test_sample_filter": (_i, [_vp, _vp, _i, _i, C.c_float, _i, C.c_float, _vp, _vp]),
 }
 
 _lib = None

@@ -210,12 +210,16 @@ struct vly_kv {
   Owned<long long> dbg;               // [SMs][32] cycle counters (StepParams::dbg); allocated only with VLY_MEGA_DBG
   Owned<SampleState> d_sample;        // token selection state read by every decode step (sampling.cuh)
   bool sample_dirty = false;          // device state is not the plain-greedy default
+  bool filtered = false;              // the last sampling set has a top-k / top-p filter: sample_filter_kernel selects
   Owned<uint32_t> key_bits;           // [B, Smax/32] attention_mask bits (1 = attend); all ones unless vly_kv_set_key_mask
   bool masked = false;
   int mask_words() const { return Smax / 32; }
   cudaGraphExec_t graph = nullptr;     // one decode step
   cudaGraphExec_t graph_n = nullptr;   // kGraphSteps steps in one graph (fewer graph launches, kernel->kernel edges inside)
   int graph_nodes = 0;
+  cudaGraphExec_t graph_f = nullptr;   // the same two with the filtered selection after every step, captured on first use
+  cudaGraphExec_t graph_fn = nullptr;
+  int graph_nodes_f = 0;
   size_t layer_stride() const { return (size_t)2 * B * ctx->cfg.num_attention_heads * Smax * 128; }
   bf16* k_layer(int l) const { return cache + (size_t)l * layer_stride(); }
   bf16* v_layer(int l) const { return k_layer(l) + layer_stride() / 2; }
@@ -224,6 +228,8 @@ struct vly_kv {
   ~vly_kv() {
     if (graph) cudaGraphExecDestroy(graph);
     if (graph_n) cudaGraphExecDestroy(graph_n);
+    if (graph_f) cudaGraphExecDestroy(graph_f);
+    if (graph_fn) cudaGraphExecDestroy(graph_fn);
     if (len_event) cudaEventDestroy(len_event);
   }
 };
@@ -1642,8 +1648,27 @@ static int launch_decode_mega(vly_ctx* c, vly_kv* kv, cudaStream_t st) {
   return VLY_OK;
 }
 
-static int enqueue_full_step(vly_ctx* c, vly_kv* kv, cudaStream_t st) {
-  if (kv->B <= 4) return launch_decode_mega(c, kv, st);
+// top-k / top-p selection over [B, V] logits (sampling.cuh), one CTA per row
+static int launch_sample_filter(vly_ctx* c, const float* logits, int B, int V, SampleState* s, const int* seq_len, const int* step,
+                                long long* next_tokens, long long* out_tokens, int out_stride, int mode, uint8_t* keep_out,
+                                cudaStream_t st) {
+  const size_t smem = (size_t)V * 4 <= (size_t)kFilterStageMaxBytes ? (size_t)V * 4 : 0;
+  TRY(ensure_smem_attr(c->cfg.device, sample_filter_kernel, smem));
+  sample_filter_kernel<<<B, kFilterThreads, smem, st>>>(logits, V, s, seq_len, step, next_tokens, out_tokens, out_stride, mode, keep_out);
+  c->launches++;
+  CKL();
+  return VLY_OK;
+}
+
+// filtered: the step's selection is sample_filter_kernel's (the decode kernels see the plain-greedy state, set_sampling)
+static int enqueue_full_step(vly_ctx* c, vly_kv* kv, cudaStream_t st, bool filtered = false) {
+  if (kv->B <= 4) {
+    TRY(launch_decode_mega(c, kv, st));
+    if (filtered)
+      TRY(launch_sample_filter(c, kv->logits, kv->B, c->cfg.vocab_size, kv->d_sample, kv->d_len, kv->d_step, kv->cur_tokens,
+                               kv->gen_tokens, kv->Smax, FILTER_AFTER_MEGA, nullptr, st));
+    return VLY_OK;
+  }
   for (int b0 = 0; b0 < kv->B; b0 += 4) {
     const int nb = (kv->B - b0) < 4 ? (kv->B - b0) : 4;
     TRY(enqueue_decode_step(c, kv, b0, nb, b0 + 4 >= kv->B, st));
@@ -1654,6 +1679,9 @@ static int enqueue_full_step(vly_ctx* c, vly_kv* kv, cudaStream_t st) {
                                            kv->gen_tokens, kv->Smax, 0);
     c->launches++;
     CKL();
+    if (filtered)
+      TRY(launch_sample_filter(c, kv->logits, kv->B, c->cfg.vocab_size, kv->d_sample, kv->d_len, kv->d_step, kv->cur_tokens,
+                               kv->gen_tokens, kv->Smax, FILTER_AFTER_PEROP, nullptr, st));
   }
   return VLY_OK;
 }
@@ -1671,15 +1699,29 @@ __global__ void set_sample_state_kernel(SampleState* s, float inv_temp, int enab
 // sampling == nullptr: plain greedy, no stop token (skipped when the device state already says so)
 static int set_sampling(vly_ctx* c, vly_kv* kv, const vly_sampling* sp, bool reset_done, cudaStream_t st) {
   if (!sp) {
+    kv->filtered = false;
     if (!kv->sample_dirty) return VLY_OK;
     set_sample_state_kernel<<<1, 64, 0, st>>>(kv->d_sample, 1.f, 0, 0, 0, -1, 0, -1, 1);
     kv->sample_dirty = false;
   } else {
     if (kv->B > kMaxSampleRows) return fail(VLY_ERR_INVALID, "sampling / eos bookkeeping supports at most %d sequences per cache", kMaxSampleRows);
     const bool on = sp->temperature >= 1e-4f;         // model_worker.py:390: below that the reference takes the arg-max
-    set_sample_state_kernel<<<1, 64, 0, st>>>(kv->d_sample, on ? 1.f / sp->temperature : 1.f, on ? 1 : 0, (uint32_t)sp->seed,
-                                              (uint32_t)(sp->seed >> 32), sp->eos_token_id < 0 ? -1 : sp->eos_token_id, sp->pad_token_id,
-                                              sp->stop_token_id < 0 ? -1 : sp->stop_token_id, reset_done ? 1 : 0);
+    const uint32_t k0 = (uint32_t)sp->seed, k1 = (uint32_t)(sp->seed >> 32);
+    const long long eos = sp->eos_token_id < 0 ? -1 : sp->eos_token_id, stop2 = sp->stop_token_id < 0 ? -1 : sp->stop_token_id;
+    // the filters apply only when sampling (HF ignores its warpers when it does not sample)
+    kv->filtered = on && (sp->top_k > 0 || (sp->top_p > 0.f && sp->top_p < 1.f));
+    if (kv->filtered) {
+      // the decode step sees plain greedy; the request goes to the filter block (a copy, not a launch: the filtered step differs
+      // from the plain one by exactly its one extra kernel)
+      SampleFilter f = {};
+      f.temperature = sp->temperature; f.inv_temp = 1.f / sp->temperature; f.top_k = sp->top_k; f.top_p = sp->top_p;
+      f.seed_lo = k0; f.seed_hi = k1; f.eos = eos; f.pad = sp->pad_token_id; f.stop2 = stop2;
+      set_sample_state_kernel<<<1, 64, 0, st>>>(kv->d_sample, 1.f, 0, 0, 0, -1, sp->pad_token_id, -1, reset_done ? 1 : 0);
+      CK(cudaMemcpyAsync(&kv->d_sample->filt, &f, sizeof(f), cudaMemcpyHostToDevice, st));   // (pageable: staged before the return)
+    } else {
+      set_sample_state_kernel<<<1, 64, 0, st>>>(kv->d_sample, on ? 1.f / sp->temperature : 1.f, on ? 1 : 0, k0, k1, eos, sp->pad_token_id,
+                                                stop2, reset_done ? 1 : 0);
+    }
     kv->sample_dirty = true;
   }
   c->launches++;
@@ -1688,14 +1730,14 @@ static int set_sampling(vly_ctx* c, vly_kv* kv, const vly_sampling* sp, bool res
 }
 
 constexpr int kGraphSteps = 8;
-static int capture_steps(vly_ctx* c, vly_kv* kv, int n, cudaGraphExec_t* out) {
+static int capture_steps(vly_ctx* c, vly_kv* kv, int n, cudaGraphExec_t* out, bool filtered = false) {
   const int64_t before = c->launches;
   CK(cudaStreamBeginCapture(c->cap_stream, cudaStreamCaptureModeThreadLocal));
   int r = VLY_OK;
-  for (int i = 0; i < n && r == VLY_OK; ++i) r = enqueue_full_step(c, kv, c->cap_stream);
+  for (int i = 0; i < n && r == VLY_OK; ++i) r = enqueue_full_step(c, kv, c->cap_stream, filtered);
   cudaGraph_t graph = nullptr;
   const cudaError_t e = cudaStreamEndCapture(c->cap_stream, &graph);
-  kv->graph_nodes = (int)((c->launches - before) / n);
+  (filtered ? kv->graph_nodes_f : kv->graph_nodes) = (int)((c->launches - before) / n);
   c->launches = before;
   if (r != VLY_OK) {
     if (graph) cudaGraphDestroy(graph);
@@ -1713,6 +1755,12 @@ static int build_graph(vly_ctx* c, vly_kv* kv) {
   TRY(capture_steps(c, kv, kGraphSteps, &kv->graph_n));
   return VLY_OK;
 }
+static int build_graph_filtered(vly_ctx* c, vly_kv* kv) {
+  if (kv->graph_f) return VLY_OK;
+  TRY(capture_steps(c, kv, 1, &kv->graph_f, true));
+  TRY(capture_steps(c, kv, kGraphSteps, &kv->graph_fn, true));
+  return VLY_OK;
+}
 
 extern "C" int vly_sample_logits(vly_ctx* c, vly_kv* kv, const float* logits, const vly_sampling* sp, int64_t* tokens_out, void* stream) {
   if (!c || !kv || !logits || !sp || !tokens_out || kv->ctx != c) return fail(VLY_ERR_INVALID, "vly_sample_logits: bad argument");
@@ -1720,6 +1768,9 @@ extern "C" int vly_sample_logits(vly_ctx* c, vly_kv* kv, const float* logits, co
   CK(cudaSetDevice(c->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   TRY(set_sampling(c, kv, sp, true, st));
+  if (kv->filtered)
+    return launch_sample_filter(c, logits, kv->B, c->cfg.vocab_size, kv->d_sample, kv->d_len, kv->d_step, (long long*)tokens_out, nullptr,
+                                0, FILTER_FIRST, nullptr, st);
   sample_rows_kernel<<<1, 1024, 0, st>>>(logits, kv->B, c->cfg.vocab_size, kv->d_sample, kv->d_len, kv->d_step, (long long*)tokens_out, nullptr, 0, 1);
   c->launches++;
   CKL();
@@ -1750,15 +1801,18 @@ static int generate_impl(vly_ctx* c, vly_kv* kv, const int64_t* first_tokens, in
   if (!no_graph) TRY(build_graph(c, kv));
   // with a sampling struct the eos flags raised by vly_sample_logits (the first token) are kept; greedy starts clean
   TRY(set_sampling(c, kv, sp, false, st));
+  const bool filtered = kv->filtered;
+  if (!no_graph && filtered) TRY(build_graph_filtered(c, kv));
+  cudaGraphExec_t one = filtered ? kv->graph_f : kv->graph, many = filtered ? kv->graph_fn : kv->graph_n;
   CK(cudaMemcpyAsync(kv->cur_tokens, first_tokens, (size_t)kv->B * 8, cudaMemcpyDeviceToDevice, st));
   CK(cudaMemsetAsync(kv->d_step, 0, 4, st));
   if (steps_done_dev) CK(cudaMemsetAsync(&kv->d_sample->steps_valid, 0, 4, st));
   for (int i = 0; i < n_steps;) {
-    if (no_graph) { TRY(enqueue_full_step(c, kv, st)); ++i; }
-    else if (kv->graph_n && n_steps - i >= kGraphSteps) { CK(cudaGraphLaunch(kv->graph_n, st)); i += kGraphSteps; }
-    else { CK(cudaGraphLaunch(kv->graph, st)); ++i; }
+    if (no_graph) { TRY(enqueue_full_step(c, kv, st, filtered)); ++i; }
+    else if (many && n_steps - i >= kGraphSteps) { CK(cudaGraphLaunch(many, st)); i += kGraphSteps; }
+    else { CK(cudaGraphLaunch(one, st)); ++i; }
   }
-  if (!no_graph) c->launches += (int64_t)n_steps * kv->graph_nodes;
+  if (!no_graph) c->launches += (int64_t)n_steps * (filtered ? kv->graph_nodes_f : kv->graph_nodes);
   if (out_tokens)
     CK(cudaMemcpy2DAsync(out_tokens, (size_t)n_steps * 8, kv->gen_tokens, (size_t)kv->Smax * 8, (size_t)n_steps * 8, kv->B,
                          cudaMemcpyDeviceToDevice, st));
@@ -1885,4 +1939,18 @@ extern "C" int vly_test_vit_attention(vly_ctx* c, const void* qkv, int F, void* 
   std::lock_guard<std::mutex> lk(c->mu);
   CK(cudaSetDevice(c->cfg.device));
   return launch_vit_attention(c, (const bf16*)qkv, F, (bf16*)out, (cudaStream_t)stream);
+}
+
+extern "C" int vly_test_sample_filter(vly_ctx* c, const float* logits, int B, int V, float temperature, int top_k, float top_p,
+                                      uint8_t* keep_out, void* stream) {
+  if (!c || !logits || !keep_out || B <= 0 || B > 65535 || V <= 0 || !(temperature > 0.f))
+    return fail(VLY_ERR_INVALID, "vly_test_sample_filter: bad argument");
+  std::lock_guard<std::mutex> lk(c->mu);
+  CK(cudaSetDevice(c->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  SampleState s = {};
+  s.filt.temperature = temperature; s.filt.inv_temp = 1.f / temperature; s.filt.top_k = top_k; s.filt.top_p = top_p;
+  TRY(ensure(c->w_score, sizeof(SampleState)));
+  CK(cudaMemcpyAsync(c->w_score.p, &s, sizeof(s), cudaMemcpyHostToDevice, st));
+  return launch_sample_filter(c, logits, B, V, (SampleState*)c->w_score.p, nullptr, nullptr, nullptr, nullptr, 0, FILTER_FIRST, keep_out, st);
 }

@@ -322,6 +322,44 @@ class KeywordsStoppingCriteria:
 _UNSET = object()
 
 
+def sampling_filters(top_k=None, top_p=None) -> Tuple[int, float]:
+    """``generate``'s ``top_k`` / ``top_p`` as HF's generate reads them when it samples (generation/utils.py builds
+    ``TopKLogitsWarper`` for ``top_k not in (None, 0)`` and ``TopPLogitsWarper`` for ``top_p`` below 1).  Returns
+    ``(top_k, top_p)`` with 0 / 1.0 meaning off and raises HF's ``ValueError`` for values its warpers reject.
+    ``top_p == 0`` is legal in HF and keeps one token: it becomes ``top_k = 1``."""
+    k, p = 0, 1.0
+    if top_k is not None and top_k != 0:
+        if not isinstance(top_k, int) or top_k <= 0:
+            raise ValueError(f"`top_k` has to be a strictly positive integer, but is {top_k}")
+        k = top_k
+    if top_p is not None:
+        top_p = float(top_p)
+        if top_p < 0 or top_p > 1.0:
+            raise ValueError(f"`top_p` has to be a float > 0 and < 1, but is {top_p}")
+        if top_p == 0.0:
+            k = 1
+        elif top_p < 1.0:
+            p = top_p
+    return k, p
+
+
+def filter_scores(scores: torch.Tensor, top_k: int, top_p: float) -> torch.Tensor:
+    """HF's ``TopKLogitsWarper`` then ``TopPLogitsWarper`` (generation/logits_process.py) on ``scores = logits / temperature``
+    [B, V] fp32, with ``(top_k, top_p)`` from ``sampling_filters``: removed tokens become -inf.  The host-visible decode loop
+    samples with it; the device loop applies the same filters in ``sample_filter_kernel``."""
+    if top_k > 0:
+        kth = torch.topk(scores, min(top_k, scores.size(-1)))[0][..., -1, None]
+        scores = scores.masked_fill(scores < kth, -float("inf"))
+    if top_p < 1.0:
+        sorted_logits, sorted_indices = torch.sort(scores, descending=False)
+        cumulative_probs = sorted_logits.softmax(dim=-1).cumsum(dim=-1)
+        sorted_indices_to_remove = cumulative_probs <= (1 - top_p)
+        sorted_indices_to_remove[..., -1:] = 0
+        indices_to_remove = sorted_indices_to_remove.scatter(1, sorted_indices, sorted_indices_to_remove)
+        scores = scores.masked_fill(indices_to_remove, -float("inf"))
+    return scores
+
+
 def _open_video_reader(path: str):
     """Default file reader of ``completion(tokenizer, path, ...)``: decord, exactly as load_video opens it
     (data_util.py:258-260).  Container decoding is CPU work outside the hot path; inject another reader factory through
@@ -678,17 +716,23 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
 
     @torch.no_grad()
     def generate(self, input_ids=None, images=None, max_new_tokens: int = 1024, do_sample: bool = False,
-                 temperature: float = 1.0, stopping_criteria=None, eos_token_id=_UNSET, **kw):
+                 temperature: float = 1.0, stopping_criteria=None, eos_token_id=_UNSET, top_k=None, top_p=None, **kw):
         """Greedy (or temperature) generation == the loop of model_worker.py:371-397 / HF generate as called at
         valley_model.py:432.  Returns [B, S + n_new] like HF.  With no stopping criteria, decoding runs
         entirely on the device (CUDA-graph replay, no per-token host sync).  ``attention_mask`` [B, S] (left padding)
         is honoured like HF generate does; generated positions are always attendable.
+
+        ``top_k`` / ``top_p`` filter the sampled distribution after the temperature, as HF's warpers do (``sampling_filters``
+        gives the argument handling).  They apply only when sampling: with ``do_sample=False`` or a temperature below 1e-4
+        they are ignored.  Unlike HF, no ``top_k = 50`` is implied when none is given.
 
         HF defaults that the reference's callers rely on are kept: ``eos_token_id`` / ``pad_token_id`` default to the config's
         (generation stops when every row has emitted eos; finished rows are padded), and when no ``attention_mask`` is given
         but the prompt contains ``pad_token_id`` (!= eos) the mask is inferred as ``input_ids != pad_token_id``
         (HF:generation/utils.py _prepare_attention_mask_for_generation).  Pass ``eos_token_id=None`` to run the full length."""
         B, S = input_ids.shape
+        greedy = (not do_sample) or temperature < 1e-4
+        filters = {} if greedy else dict(zip(("top_k", "top_p"), sampling_filters(top_k, top_p)))
         room = self.config.max_position_embeddings - S
         n_new = max(0, min(max_new_tokens, room))
         if n_new == 0:
@@ -706,12 +750,12 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
         try:
             cache.set_attention_mask(attention_mask, S)
             return self._generate_with_cache(cache, input_ids, embeds, n_new, do_sample, temperature, stopping_criteria, eos_token_id,
-                                             pad_token_id)
+                                             pad_token_id, **filters)
         finally:
             self._return_cache(cache)
 
     def _generate_with_cache(self, cache, input_ids, embeds, n_new, do_sample, temperature, stopping_criteria, eos_token_id,
-                             pad_token_id=None):
+                             pad_token_id=None, top_k=0, top_p=1.0):
         B = input_ids.shape[0]
         greedy = (not do_sample) or temperature < 1e-4
         device_select = not stopping_criteria and not (greedy and eos_token_id is None) and B <= 64
@@ -731,7 +775,8 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
             eos = -1 if eos_token_id is None else int(eos_token_id)
             pad = int(pad_token_id) if pad_token_id is not None else max(eos, 0)      # HF: pad defaults to eos
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())                         # torch.manual_seed() governs it
-            sp = VlySampling(0.0 if greedy else float(temperature), seed, eos, pad)
+            # (a top-k / top-p filter: one more kernel per step selects over the step's logits, still on the device)
+            sp = VlySampling(0.0 if greedy else float(temperature), seed, eos, pad, top_k=top_k, top_p=top_p)
             out = torch.empty(B, n_new, dtype=torch.int64, device=self.device)
             first = torch.empty(B, dtype=torch.int64, device=self.device)
             check(self._lib.vly_sample_logits(self._ctx, cache._h, logits.data_ptr(), C.byref(sp), first.data_ptr(), _stream()))
@@ -752,7 +797,8 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
         pad = int(pad_token_id) if pad_token_id is not None else (int(eos_token_id) if eos_token_id is not None else 0)
         for i in range(n_new):
             if not greedy:
-                probs = torch.softmax(logits[:, -1, :] / temperature, dim=-1)    # model_worker.py:393-394
+                scores = filter_scores(logits[:, -1, :] / temperature, top_k, top_p)     # model_worker.py:393-394
+                probs = torch.softmax(scores, dim=-1)
                 nxt = torch.multinomial(probs, num_samples=1).reshape(B)
             if eos_token_id is not None:
                 nxt = torch.where(finished, torch.full_like(nxt, pad), nxt)

@@ -21,7 +21,7 @@ import torch
 
 from ._lib import VlySampling, check
 from .model import (DEFAULT_IM_END_TOKEN, DEFAULT_IM_START_TOKEN, DEFAULT_IMAGE_PATCH_TOKEN, DEFAULT_VI_END_TOKEN,
-                    DEFAULT_VI_START_TOKEN, DEFAULT_VIDEO_FRAME_TOKEN)
+                    DEFAULT_VI_START_TOKEN, DEFAULT_VIDEO_FRAME_TOKEN, sampling_filters)
 
 DEFAULT_VIDEO_TOKEN = "<video>"          # valley/util/config.py
 
@@ -54,7 +54,8 @@ def generate_stream(model, tokenizer, params: Dict, *, context_len: int = 2048, 
     """Yields ``{"text": ori_prompt + text_so_far, "error_code": 0}`` exactly when the reference worker does.
 
     params: "prompt", optional "video" ([T,3,224,224] pixel tensor, already preprocessed -- see valley_b200.video), "temperature"
-    (default 1.0), "max_new_tokens" (default 256, capped at 1024), "stop"."""
+    (default 1.0), "max_new_tokens" (default 256, capped at 1024), "stop", and "top_k" / "top_p" (HF generate's filters, as
+    ``ValleyLlamaForCausalLM.generate`` takes them; absent: no filter)."""
     prompt = params["prompt"]
     ori_prompt = prompt
     video = params.get("video", None)
@@ -65,6 +66,7 @@ def generate_stream(model, tokenizer, params: Dict, *, context_len: int = 2048, 
         prompt = expand_video_prompt(prompt, video.shape[0], getattr(model.config, "mm_use_im_start_end", False))
         images = video.to(model.device, torch.float16).unsqueeze(0)                                        # :335-336, :345
     temperature = float(params.get("temperature", 1.0))
+    top_k, top_p = sampling_filters(params.get("top_k"), params.get("top_p")) if temperature >= 1e-4 else (0, 1.0)
     max_new_tokens = min(int(params.get("max_new_tokens", 256)), 1024)
     stop_str = params.get("stop", None)
     stop_idx = stop_token_index(tokenizer, stop_str)
@@ -82,7 +84,7 @@ def generate_stream(model, tokenizer, params: Dict, *, context_len: int = 2048, 
     try:
         logits, _ = model._prefill(cache, embeds, 1)
         sp = VlySampling(temperature if temperature >= 1e-4 else 0.0, int(torch.randint(0, 2 ** 62, (1,)).item()),
-                         -1 if eos is None else int(eos), 0, -1 if stop_idx is None else int(stop_idx))
+                         -1 if eos is None else int(eos), 0, -1 if stop_idx is None else int(stop_idx), top_k, top_p)
         st = torch.cuda.current_stream(model.device).cuda_stream
         tok = torch.empty(1, dtype=torch.int64, device=model.device)
         check(model._lib.vly_sample_logits(model._ctx, cache._h, logits.data_ptr(), C.byref(sp), tok.data_ptr(), st))
