@@ -164,7 +164,7 @@ def _gen(m, ids, px, n, seed, **kw):
 @pytest.mark.gpu
 @pytest.mark.parametrize("B", [1, 2, 6])
 def test_a_filter_that_keeps_everything_draws_the_unfiltered_tokens(B):
-    """top_k = V runs the filtered selection (one more kernel per step) and must draw bit for bit what the unfiltered sampler
+    """top_k = V runs the filtered selection and must draw bit for bit what the unfiltered sampler
     draws with the same seed: the first token, the persistent kernel (B <= 4) and the per-op kernels (B = 6)."""
     spec, m = get("tiny")
     V = spec.vocab_size
@@ -230,7 +230,9 @@ def test_eos_under_a_filter_stops_and_pads_rows(B):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("B", [2, 6])
-def test_a_filtered_step_launches_one_more_kernel_and_allocates_nothing(B):
+def test_a_filtered_step_adds_a_kernel_only_after_the_persistent_kernel_and_allocates_nothing(B):
+    """the persistent kernel (B <= 4) leaves a filtered selection to one more kernel; the per-op path (B > 4) selects in a
+    kernel of its own either way"""
     from test_gpu_ownership import held
     spec, m = get("tiny")
     ids, px = syn.make_prompt_ids(spec, B, 2, 3), syn.make_pixels(B, 2, 3)
@@ -250,7 +252,7 @@ def test_a_filtered_step_launches_one_more_kernel_and_allocates_nothing(B):
     h0 = held()
     filt = per_step(do_sample=True, temperature=0.8, top_k=40)      # the first filtered generate on this cache captures its graphs
     assert held() == h0
-    assert plain == greedy and filt == plain + 1, (greedy, plain, filt)
+    assert plain == greedy and filt == plain + (1 if B <= 4 else 0), (greedy, plain, filt)
     _gen(m, ids, px, 9, 6, do_sample=True, temperature=0.8, top_p=0.5)
     assert held() == h0
 

@@ -214,22 +214,19 @@ struct vly_kv {
   Owned<uint32_t> key_bits;           // [B, Smax/32] attention_mask bits (1 = attend); all ones unless vly_kv_set_key_mask
   bool masked = false;
   int mask_words() const { return Smax / 32; }
-  cudaGraphExec_t graph = nullptr;     // one decode step
-  cudaGraphExec_t graph_n = nullptr;   // kGraphSteps steps in one graph (fewer graph launches, kernel->kernel edges inside)
-  int graph_nodes = 0;
-  cudaGraphExec_t graph_f = nullptr;   // the same two with the filtered selection after every step, captured on first use
-  cudaGraphExec_t graph_fn = nullptr;
-  int graph_nodes_f = 0;
+  // the decode step as CUDA graphs, [filtered][0: one step, 1: kGraphSteps steps in one graph (fewer graph launches,
+  // kernel->kernel edges inside)]; each pair is captured on first use
+  cudaGraphExec_t graph[2][2] = {};
+  int graph_nodes[2] = {};            // kernel launches per step of each pair
   size_t layer_stride() const { return (size_t)2 * B * ctx->cfg.num_attention_heads * Smax * 128; }
   bf16* k_layer(int l) const { return cache + (size_t)l * layer_stride(); }
   bf16* v_layer(int l) const { return k_layer(l) + layer_stride() / 2; }
 
   // (runs before the buffers the graphs and the event refer to are freed)
   ~vly_kv() {
-    if (graph) cudaGraphExecDestroy(graph);
-    if (graph_n) cudaGraphExecDestroy(graph_n);
-    if (graph_f) cudaGraphExecDestroy(graph_f);
-    if (graph_fn) cudaGraphExecDestroy(graph_fn);
+    for (auto& pair : graph)
+      for (cudaGraphExec_t g : pair)
+        if (g) cudaGraphExecDestroy(g);
     if (len_event) cudaEventDestroy(len_event);
   }
 };
@@ -1319,8 +1316,7 @@ extern "C" int vly_kv_create(vly_ctx* c, int batch, int max_seq, vly_kv** out) {
   TRY(kv->gen_tokens.alloc((size_t)batch * kv->Smax * 8));
   TRY(kv->d_sample.alloc(sizeof(SampleState)));
   {
-    SampleState s0 = {};
-    s0.inv_temp = 1.f; s0.eos = -1; s0.pad = 0; s0.stop2 = -1;
+    const SampleState s0 = {};
     CK(cudaMemcpy(kv->d_sample, &s0, sizeof(s0), cudaMemcpyHostToDevice));
   }
   TRY(kv->key_bits.alloc((size_t)batch * kv->mask_words() * 4));
@@ -1629,10 +1625,12 @@ extern "C" int vly_kv_debug_counters(vly_kv* kv, long long* host_out, int n) {
   return VLY_OK;
 }
 
-// the launch was planned by vly_kv_create (plan_decode_mega)
-static int launch_decode_mega(vly_ctx* c, vly_kv* kv, cudaStream_t st) {
+// the launch was planned by vly_kv_create (plan_decode_mega); filtered: sample_filter_kernel selects after the step
+static int launch_decode_mega(vly_ctx* c, vly_kv* kv, bool filtered, cudaStream_t st) {
   const int bmax = kv->B <= 1 ? 1 : (kv->B <= 2 ? 2 : 4);
-  void* args[] = {&kv->mega};
+  StepParams p = kv->mega;
+  p.select = filtered ? 0 : 1;
+  void* args[] = {&p};
   cudaError_t e;
 #define VLY_MEGA_CASE(BM)                                                                                                          \
   {                                                                                                                                \
@@ -1648,49 +1646,44 @@ static int launch_decode_mega(vly_ctx* c, vly_kv* kv, cudaStream_t st) {
   return VLY_OK;
 }
 
-// top-k / top-p selection over [B, V] logits (sampling.cuh), one CTA per row
+// token selection over [B, V] logits (sampling.cuh), one CTA per row; the scores of a filtered row are staged in shared memory
 static int launch_sample_filter(vly_ctx* c, const float* logits, int B, int V, SampleState* s, const int* seq_len, const int* step,
-                                long long* next_tokens, long long* out_tokens, int out_stride, int mode, uint8_t* keep_out,
-                                cudaStream_t st) {
-  const size_t smem = (size_t)V * 4 <= (size_t)kFilterStageMaxBytes ? (size_t)V * 4 : 0;
+                                long long* next_tokens, long long* out_tokens, int out_stride, bool filter, bool per_op,
+                                uint8_t* keep_out, cudaStream_t st) {
+  const size_t smem = filter && (size_t)V * 4 <= (size_t)kFilterStageMaxBytes ? (size_t)V * 4 : 0;
   TRY(ensure_smem_attr(c->cfg.device, sample_filter_kernel, smem));
-  sample_filter_kernel<<<B, kFilterThreads, smem, st>>>(logits, V, s, seq_len, step, next_tokens, out_tokens, out_stride, mode, keep_out);
+  sample_filter_kernel<<<B, kFilterThreads, smem, st>>>(logits, V, s, seq_len, step, next_tokens, out_tokens, out_stride, filter ? 1 : 0,
+                                                        per_op ? 1 : 0, keep_out);
   c->launches++;
   CKL();
   return VLY_OK;
 }
 
-// filtered: the step's selection is sample_filter_kernel's (the decode kernels see the plain-greedy state, set_sampling)
-static int enqueue_full_step(vly_ctx* c, vly_kv* kv, cudaStream_t st, bool filtered = false) {
+// filtered: the step ends with sample_filter_kernel's filtered selection (set_sampling)
+static int enqueue_full_step(vly_ctx* c, vly_kv* kv, bool filtered, cudaStream_t st) {
   if (kv->B <= 4) {
-    TRY(launch_decode_mega(c, kv, st));
+    TRY(launch_decode_mega(c, kv, filtered, st));
     if (filtered)
       TRY(launch_sample_filter(c, kv->logits, kv->B, c->cfg.vocab_size, kv->d_sample, kv->d_len, kv->d_step, kv->cur_tokens,
-                               kv->gen_tokens, kv->Smax, FILTER_AFTER_MEGA, nullptr, st));
+                               kv->gen_tokens, kv->Smax, true, false, nullptr, st));
     return VLY_OK;
   }
   for (int b0 = 0; b0 < kv->B; b0 += 4) {
     const int nb = (kv->B - b0) < 4 ? (kv->B - b0) : 4;
     TRY(enqueue_decode_step(c, kv, b0, nb, b0 + 4 >= kv->B, st));
   }
-  // per-op paths: temperature sampling / eos bookkeeping as one more launch over the step's logits (returns at once when greedy)
-  if (kv->B <= kMaxSampleRows) {
-    sample_rows_kernel<<<1, 1024, 0, st>>>(kv->logits, kv->B, c->cfg.vocab_size, kv->d_sample, kv->d_len, kv->d_step, kv->cur_tokens,
-                                           kv->gen_tokens, kv->Smax, 0);
-    c->launches++;
-    CKL();
-    if (filtered)
-      TRY(launch_sample_filter(c, kv->logits, kv->B, c->cfg.vocab_size, kv->d_sample, kv->d_len, kv->d_step, kv->cur_tokens,
-                               kv->gen_tokens, kv->Smax, FILTER_AFTER_PEROP, nullptr, st));
-  }
+  // per-op paths: sampling / eos bookkeeping as one more launch over the step's logits (returns at once when greedy)
+  if (kv->B <= kMaxSampleRows)
+    TRY(launch_sample_filter(c, kv->logits, kv->B, c->cfg.vocab_size, kv->d_sample, kv->d_len, kv->d_step, kv->cur_tokens,
+                             kv->gen_tokens, kv->Smax, filtered, true, nullptr, st));
   return VLY_OK;
 }
 
 // ---- token selection state ----
-__global__ void set_sample_state_kernel(SampleState* s, float inv_temp, int enabled, uint32_t k0, uint32_t k1, long long eos, long long pad,
-                                        long long stop2, int reset_done) {
+__global__ void set_sample_state_kernel(SampleState* s, const SampleState r, int reset_done) {
   if (threadIdx.x == 0) {
-    s->inv_temp = inv_temp; s->enabled = enabled; s->seed_lo = k0; s->seed_hi = k1; s->eos = eos; s->pad = pad; s->stop2 = stop2;
+    s->temperature = r.temperature; s->inv_temp = r.inv_temp; s->enabled = r.enabled; s->top_k = r.top_k; s->top_p = r.top_p;
+    s->seed_lo = r.seed_lo; s->seed_hi = r.seed_hi; s->eos = r.eos; s->pad = r.pad; s->stop2 = r.stop2;
     if (reset_done) { s->all_done = 0; s->steps_valid = 0; }
   }
   if (reset_done && threadIdx.x < kMaxSampleRows) s->done[threadIdx.x] = 0;
@@ -1698,46 +1691,40 @@ __global__ void set_sample_state_kernel(SampleState* s, float inv_temp, int enab
 
 // sampling == nullptr: plain greedy, no stop token (skipped when the device state already says so)
 static int set_sampling(vly_ctx* c, vly_kv* kv, const vly_sampling* sp, bool reset_done, cudaStream_t st) {
+  SampleState r = {};
+  kv->filtered = false;
   if (!sp) {
-    kv->filtered = false;
     if (!kv->sample_dirty) return VLY_OK;
-    set_sample_state_kernel<<<1, 64, 0, st>>>(kv->d_sample, 1.f, 0, 0, 0, -1, 0, -1, 1);
-    kv->sample_dirty = false;
+    reset_done = true;
   } else {
     if (kv->B > kMaxSampleRows) return fail(VLY_ERR_INVALID, "sampling / eos bookkeeping supports at most %d sequences per cache", kMaxSampleRows);
     const bool on = sp->temperature >= 1e-4f;         // model_worker.py:390: below that the reference takes the arg-max
-    const uint32_t k0 = (uint32_t)sp->seed, k1 = (uint32_t)(sp->seed >> 32);
-    const long long eos = sp->eos_token_id < 0 ? -1 : sp->eos_token_id, stop2 = sp->stop_token_id < 0 ? -1 : sp->stop_token_id;
+    if (on) {
+      r.temperature = sp->temperature; r.inv_temp = 1.f / sp->temperature; r.enabled = 1; r.top_k = sp->top_k; r.top_p = sp->top_p;
+    }
+    r.seed_lo = (uint32_t)sp->seed; r.seed_hi = (uint32_t)(sp->seed >> 32);
+    r.eos = sp->eos_token_id < 0 ? -1 : sp->eos_token_id;
+    r.pad = sp->pad_token_id;
+    r.stop2 = sp->stop_token_id < 0 ? -1 : sp->stop_token_id;
     // the filters apply only when sampling (HF ignores its warpers when it does not sample)
     kv->filtered = on && (sp->top_k > 0 || (sp->top_p > 0.f && sp->top_p < 1.f));
-    if (kv->filtered) {
-      // the decode step sees plain greedy; the request goes to the filter block (a copy, not a launch: the filtered step differs
-      // from the plain one by exactly its one extra kernel)
-      SampleFilter f = {};
-      f.temperature = sp->temperature; f.inv_temp = 1.f / sp->temperature; f.top_k = sp->top_k; f.top_p = sp->top_p;
-      f.seed_lo = k0; f.seed_hi = k1; f.eos = eos; f.pad = sp->pad_token_id; f.stop2 = stop2;
-      set_sample_state_kernel<<<1, 64, 0, st>>>(kv->d_sample, 1.f, 0, 0, 0, -1, sp->pad_token_id, -1, reset_done ? 1 : 0);
-      CK(cudaMemcpyAsync(&kv->d_sample->filt, &f, sizeof(f), cudaMemcpyHostToDevice, st));   // (pageable: staged before the return)
-    } else {
-      set_sample_state_kernel<<<1, 64, 0, st>>>(kv->d_sample, on ? 1.f / sp->temperature : 1.f, on ? 1 : 0, k0, k1, eos, sp->pad_token_id,
-                                                stop2, reset_done ? 1 : 0);
-    }
-    kv->sample_dirty = true;
   }
+  set_sample_state_kernel<<<1, 64, 0, st>>>(kv->d_sample, r, reset_done ? 1 : 0);
+  kv->sample_dirty = sp != nullptr;
   c->launches++;
   CKL();
   return VLY_OK;
 }
 
 constexpr int kGraphSteps = 8;
-static int capture_steps(vly_ctx* c, vly_kv* kv, int n, cudaGraphExec_t* out, bool filtered = false) {
+static int capture_steps(vly_ctx* c, vly_kv* kv, int n, bool filtered, cudaGraphExec_t* out) {
   const int64_t before = c->launches;
   CK(cudaStreamBeginCapture(c->cap_stream, cudaStreamCaptureModeThreadLocal));
   int r = VLY_OK;
-  for (int i = 0; i < n && r == VLY_OK; ++i) r = enqueue_full_step(c, kv, c->cap_stream, filtered);
+  for (int i = 0; i < n && r == VLY_OK; ++i) r = enqueue_full_step(c, kv, filtered, c->cap_stream);
   cudaGraph_t graph = nullptr;
   const cudaError_t e = cudaStreamEndCapture(c->cap_stream, &graph);
-  (filtered ? kv->graph_nodes_f : kv->graph_nodes) = (int)((c->launches - before) / n);
+  kv->graph_nodes[filtered] = (int)((c->launches - before) / n);
   c->launches = before;
   if (r != VLY_OK) {
     if (graph) cudaGraphDestroy(graph);
@@ -1749,16 +1736,11 @@ static int capture_steps(vly_ctx* c, vly_kv* kv, int n, cudaGraphExec_t* out, bo
   if (e2 != cudaSuccess) return fail(VLY_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(e2));
   return VLY_OK;
 }
-static int build_graph(vly_ctx* c, vly_kv* kv) {
-  if (kv->graph) return VLY_OK;
-  TRY(capture_steps(c, kv, 1, &kv->graph));
-  TRY(capture_steps(c, kv, kGraphSteps, &kv->graph_n));
-  return VLY_OK;
-}
-static int build_graph_filtered(vly_ctx* c, vly_kv* kv) {
-  if (kv->graph_f) return VLY_OK;
-  TRY(capture_steps(c, kv, 1, &kv->graph_f, true));
-  TRY(capture_steps(c, kv, kGraphSteps, &kv->graph_fn, true));
+static int build_graph(vly_ctx* c, vly_kv* kv, bool filtered) {
+  cudaGraphExec_t* g = kv->graph[filtered];
+  if (g[0]) return VLY_OK;
+  TRY(capture_steps(c, kv, 1, filtered, &g[0]));
+  TRY(capture_steps(c, kv, kGraphSteps, filtered, &g[1]));
   return VLY_OK;
 }
 
@@ -1768,13 +1750,8 @@ extern "C" int vly_sample_logits(vly_ctx* c, vly_kv* kv, const float* logits, co
   CK(cudaSetDevice(c->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   TRY(set_sampling(c, kv, sp, true, st));
-  if (kv->filtered)
-    return launch_sample_filter(c, logits, kv->B, c->cfg.vocab_size, kv->d_sample, kv->d_len, kv->d_step, (long long*)tokens_out, nullptr,
-                                0, FILTER_FIRST, nullptr, st);
-  sample_rows_kernel<<<1, 1024, 0, st>>>(logits, kv->B, c->cfg.vocab_size, kv->d_sample, kv->d_len, kv->d_step, (long long*)tokens_out, nullptr, 0, 1);
-  c->launches++;
-  CKL();
-  return VLY_OK;
+  return launch_sample_filter(c, logits, kv->B, c->cfg.vocab_size, kv->d_sample, kv->d_len, kv->d_step, (long long*)tokens_out, nullptr,
+                              0, kv->filtered, false, nullptr, st);
 }
 
 static int generate_impl(vly_ctx* c, vly_kv* kv, const int64_t* first_tokens, int n_steps, int64_t* out_tokens, const vly_sampling* sp,
@@ -1798,21 +1775,20 @@ static int generate_impl(vly_ctx* c, vly_kv* kv, const int64_t* first_tokens, in
   CK(cudaSetDevice(c->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   static const bool no_graph = getenv("VLY_NO_GRAPH") != nullptr;   // profiling aid: eager launches instead of graph replay
-  if (!no_graph) TRY(build_graph(c, kv));
   // with a sampling struct the eos flags raised by vly_sample_logits (the first token) are kept; greedy starts clean
   TRY(set_sampling(c, kv, sp, false, st));
   const bool filtered = kv->filtered;
-  if (!no_graph && filtered) TRY(build_graph_filtered(c, kv));
-  cudaGraphExec_t one = filtered ? kv->graph_f : kv->graph, many = filtered ? kv->graph_fn : kv->graph_n;
+  if (!no_graph) TRY(build_graph(c, kv, filtered));
+  cudaGraphExec_t one = kv->graph[filtered][0], many = kv->graph[filtered][1];
   CK(cudaMemcpyAsync(kv->cur_tokens, first_tokens, (size_t)kv->B * 8, cudaMemcpyDeviceToDevice, st));
   CK(cudaMemsetAsync(kv->d_step, 0, 4, st));
   if (steps_done_dev) CK(cudaMemsetAsync(&kv->d_sample->steps_valid, 0, 4, st));
   for (int i = 0; i < n_steps;) {
-    if (no_graph) { TRY(enqueue_full_step(c, kv, st, filtered)); ++i; }
+    if (no_graph) { TRY(enqueue_full_step(c, kv, filtered, st)); ++i; }
     else if (many && n_steps - i >= kGraphSteps) { CK(cudaGraphLaunch(many, st)); i += kGraphSteps; }
     else { CK(cudaGraphLaunch(one, st)); ++i; }
   }
-  if (!no_graph) c->launches += (int64_t)n_steps * (filtered ? kv->graph_nodes_f : kv->graph_nodes);
+  if (!no_graph) c->launches += (int64_t)n_steps * kv->graph_nodes[filtered];
   if (out_tokens)
     CK(cudaMemcpy2DAsync(out_tokens, (size_t)n_steps * 8, kv->gen_tokens, (size_t)kv->Smax * 8, (size_t)n_steps * 8, kv->B,
                          cudaMemcpyDeviceToDevice, st));
@@ -1834,12 +1810,12 @@ extern "C" int vly_llama_decode(vly_ctx* c, vly_kv* kv, const int64_t* tokens, i
   if (kv->host_len + 1 > kv->Smax) return fail(VLY_ERR_INVALID, "vly_llama_decode: cache full (%d)", kv->Smax);
   CK(cudaSetDevice(c->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  TRY(build_graph(c, kv));
+  TRY(build_graph(c, kv, false));
   TRY(set_sampling(c, kv, nullptr, true, st));
   CK(cudaMemcpyAsync(kv->cur_tokens, tokens, (size_t)kv->B * 8, cudaMemcpyDeviceToDevice, st));
   CK(cudaMemsetAsync(kv->d_step, 0, 4, st));
-  CK(cudaGraphLaunch(kv->graph, st));
-  c->launches += kv->graph_nodes;
+  CK(cudaGraphLaunch(kv->graph[0][0], st));
+  c->launches += kv->graph_nodes[0];
   if (next_tokens) CK(cudaMemcpyAsync(next_tokens, kv->cur_tokens, (size_t)kv->B * 8, cudaMemcpyDeviceToDevice, st));
   if (logits_dev) CK(cudaMemcpyAsync(logits_dev, kv->logits, (size_t)kv->B * c->cfg.vocab_size * 4, cudaMemcpyDeviceToDevice, st));
   kv->host_len += 1;
@@ -1949,8 +1925,8 @@ extern "C" int vly_test_sample_filter(vly_ctx* c, const float* logits, int B, in
   CK(cudaSetDevice(c->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   SampleState s = {};
-  s.filt.temperature = temperature; s.filt.inv_temp = 1.f / temperature; s.filt.top_k = top_k; s.filt.top_p = top_p;
+  s.temperature = temperature; s.inv_temp = 1.f / temperature; s.enabled = 1; s.top_k = top_k; s.top_p = top_p;
   TRY(ensure(c->w_score, sizeof(SampleState)));
   CK(cudaMemcpyAsync(c->w_score.p, &s, sizeof(s), cudaMemcpyHostToDevice, st));
-  return launch_sample_filter(c, logits, B, V, (SampleState*)c->w_score.p, nullptr, nullptr, nullptr, nullptr, 0, FILTER_FIRST, keep_out, st);
+  return launch_sample_filter(c, logits, B, V, (SampleState*)c->w_score.p, nullptr, nullptr, nullptr, nullptr, 0, true, false, keep_out, st);
 }

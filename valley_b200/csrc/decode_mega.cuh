@@ -78,6 +78,8 @@ struct StepParams {
   long long* dbg;               // optional [gridDim][32] cycle counters: [0..3] sync, stage-x, weight loop, attention totals;
                                 // [8 + 3*type + {0,1,2}] = stage-x, loop, trailing grid sync of every phase of that PhaseType;
                                 // [26 + type] = cycles the producer waited for a free ring slot while filling that PhaseType
+  int select;                   // 1: the last phase selects the tokens; 0: it writes the logits and a provisional arg-max, and
+                                // sample_filter_kernel selects after the step (a top-k / top-p request)
 };
 
 struct MegaCfg {
@@ -378,42 +380,33 @@ VLY_DEVINL void mega_unit_epilogue(const StepParams& p, const PhaseDesc& d, cons
   }
 }
 
-// ---- greedy arg-max over the per-CTA partials (lowest index on ties, like torch.argmax); advance the counters.
+// ---- arg-max over the per-CTA partials (lowest index on ties, like torch.argmax); advance the counters.
 // Executed by the 16 compute warps of CTA 0 after the last grid barrier of the step. ----
 VLY_DEVINL void mega_finish_step(const StepParams& p, const int cw, const int lane, const int ct) {
-      if (cw < p.B) {
-        const int b = cw;
-        float bv = -INFINITY;
-        int bi = 0x7fffffff;
-        for (int g = lane; g < (int)gridDim.x; g += 32) {
-          const float v = __ldcg(p.part_val + (size_t)b * gridDim.x + g);
-          const int i = __ldcg(p.part_idx + (size_t)b * gridDim.x + g);
-          if (v > bv || (v == bv && i < bi)) { bv = v; bi = i; }
-        }
-  #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-          const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-          const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-          if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-        }
-        if (lane == 0) {
-          const long long tok = sample_finish_row(p.sample, b, bi);
-          p.next_tokens[b] = tok;
-          if (p.out_tokens != nullptr) p.out_tokens[(size_t)b * p.out_stride + *p.step] = tok;
-        }
-      }
-      asm volatile("bar.sync 7, 512;" ::: "memory");
-      if (ct == 0) {
-        *p.step += 1;
-        *p.seq_len += 1;
-        *p.grid_epoch += 1;          // every CTA has passed the last barrier of this launch (they read the epoch at their start)
-        p.sample->steps_valid += 1;
-        if (p.sample->eos >= 0 || p.sample->stop2 >= 0) {
-          int all = 1;
-          for (int b = 0; b < p.B; ++b) all &= p.sample->done[b];
-          p.sample->all_done = all;
-        }
-      }
+  if (cw < p.B) {
+    const int b = cw;
+    float bv = -INFINITY;
+    int bi = 0x7fffffff;
+    for (int g = lane; g < (int)gridDim.x; g += 32) {
+      const float v = __ldcg(p.part_val + (size_t)b * gridDim.x + g);
+      const int i = __ldcg(p.part_idx + (size_t)b * gridDim.x + g);
+      if (v > bv || (v == bv && i < bi)) { bv = v; bi = i; }
+    }
+    warp_argmax(bv, bi);
+    if (lane == 0) {
+      const long long tok = p.select ? sample_finish_row(p.sample, b, bi) : bi;
+      p.next_tokens[b] = tok;
+      if (p.out_tokens != nullptr) p.out_tokens[(size_t)b * p.out_stride + *p.step] = tok;
+    }
+  }
+  asm volatile("bar.sync 7, 512;" ::: "memory");
+  if (ct == 0) {
+    *p.step += 1;
+    *p.seq_len += 1;
+    *p.grid_epoch += 1;          // every CTA has passed the last barrier of this launch (they read the epoch at their start)
+    if (p.select) sample_close_step(p.sample, p.B, true);
+    else p.sample->steps_valid += 1;   // (sample_filter_kernel keeps done / all_done)
+  }
 }
 
 template <int BMAX>
@@ -528,7 +521,7 @@ __global__ void __launch_bounds__(576, 1) decode_step_kernel(const StepParams p)
   const int ct = tid - 32;            // compute thread 0..511 (finalize warp: 512..543)
   const int cw = warp - 1;            // compute warp 0..15
   const int pos = *p.seq_len;
-  const bool samp_on = p.sample->enabled != 0;
+  const bool samp_on = p.select && p.sample->enabled != 0;
   const float samp_it = p.sample->inv_temp;
   const uint32_t samp_k0 = p.sample->seed_lo, samp_k1 = p.sample->seed_hi;
   unsigned int sync_no = 0;

@@ -16,35 +16,27 @@
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
+#include "common.cuh"
 
 namespace vly {
 
 constexpr int kMaxSampleRows = 64;
 
-// A request with a top-k / top-p filter (HF's TopKLogitsWarper / TopPLogitsWarper).  Such a request is selected by
-// sample_filter_kernel after the decode step, not in the step's arg-max epilogue: the step then sees the plain-greedy state
-// (enabled 0, no stop ids), and this block holds the request.  Written by the host (set_sampling).
-struct SampleFilter {
-  float temperature;          // s = logits / temperature, an IEEE fp32 division as in HF's TemperatureLogitsWarper
-  float inv_temp;             // the draw: sample_score(logit, inv_temp, ...), the same Gumbel-max as the unfiltered sampler
-  int top_k;                  // <= 0: off; >= V keeps every token
-  float top_p;                // off unless 0 < top_p < 1
-  uint32_t seed_lo, seed_hi;
-  long long eos, pad, stop2;  // < 0: none (as in SampleState)
-};
-
 struct SampleState {          // lives in device memory next to the KV cache; read by every decode step
-  float inv_temp;             // 1 / temperature
-  int enabled;                // 0 = greedy (scores are the raw logits: bit-identical to the plain arg-max)
-  uint32_t seed_lo, seed_hi;
-  long long eos, pad;         // eos < 0: no stop token
-  long long stop2;            // second stop id (the worker's single-token stop string, model_worker.py:355-360); < 0: none
-  int all_done;               // every row has produced eos: further steps exit at once
-  int steps_valid;            // decode steps executed before all_done was raised (the one that raised it included)
-  int done[kMaxSampleRows];
-  // (appended: the fields above keep their offsets, so the decode kernels that read them are unchanged)
-  SampleFilter filt;          // the filtered request (sample_filter_kernel)
-  unsigned int filt_arrive;   // CTAs of the running sample_filter_kernel that have finished their row; 0 between launches
+  // the request, written by the host (set_sampling); the defaults are plain greedy with no stop token
+  float temperature = 1.f;    // filtered scores are logits / temperature, an IEEE fp32 division as in HF's TemperatureLogitsWarper
+  float inv_temp = 1.f;       // 1 / temperature: the draw, sample_score(logit, inv_temp, ...)
+  int enabled = 0;            // 0 = greedy (scores are the raw logits: bit-identical to the plain arg-max)
+  int top_k = 0;              // top-k filter: <= 0 off; >= V keeps every token
+  float top_p = 1.f;          // top-p filter: off unless 0 < top_p < 1
+  uint32_t seed_lo = 0, seed_hi = 0;
+  long long eos = -1, pad = 0;  // eos < 0: no stop token
+  long long stop2 = -1;       // second stop id (the worker's single-token stop string, model_worker.py:355-360); < 0: none
+  // the generation's progress
+  int all_done = 0;           // every row has produced eos: further steps exit at once
+  int steps_valid = 0;        // decode steps executed before all_done was raised (the one that raised it included)
+  unsigned int arrive = 0;    // CTAs of the running sample_filter_kernel that have finished their row; 0 between launches
+  int done[kMaxSampleRows] = {};
 };
 
 __device__ __forceinline__ uint32_t philox4x32_10_first(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0, uint32_t k1) {
@@ -75,77 +67,18 @@ __device__ __forceinline__ long long sample_finish_row(SampleState* s, int b, lo
   return tok;
 }
 
-// Stand-alone selection over a [B, V] fp32 logits block: the first token after a prefill (reset = 1), and the post-step
-// selection of the per-op decode paths (B > 4).  One CTA; rows are handled one after the other.
-//   pos = *seq_len - 1 : position of the query token that produced these logits
-__global__ void __launch_bounds__(1024) sample_rows_kernel(const float* __restrict__ logits, int B, int V, SampleState* s,
-                                                           const int* seq_len, const int* step, long long* next_tokens,
-                                                           long long* out_tokens, int out_stride, int reset) {
-  __shared__ float sv[32];
-  __shared__ int si[32];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (reset) {
-    if (tid < kMaxSampleRows) s->done[tid] = 0;
-    if (tid == 0) { s->all_done = 0; s->steps_valid = 0; }
-    __syncthreads();
-  } else {
-    if (!s->enabled && s->eos < 0 && s->stop2 < 0) return;   // plain greedy: the arg-max epilogue already wrote the token
-    if (s->all_done) {                              // every row finished earlier: keep emitting pad
-      if (tid < B) {
-        next_tokens[tid] = s->pad;
-        if (out_tokens) out_tokens[(size_t)tid * out_stride + (*step - 1)] = s->pad;
-      }
-      return;
-    }
-  }
-  const int pos = *seq_len - 1;
-  const bool on = s->enabled != 0;
-  const float it = s->inv_temp;
-  const uint32_t k0 = s->seed_lo, k1 = s->seed_hi;
-  for (int b = 0; b < B; ++b) {
-    float bv = -INFINITY;
-    int bi = 0x7fffffff;
-    for (int n = tid; n < V; n += 1024) {
-      const float y = logits[(size_t)b * V + n];
-      const float v = on ? sample_score(y, it, k0, k1, n, b, pos) : y;
-      if (v > bv) { bv = v; bi = n; }               // ascending n per thread: first maximum kept
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-    }
-    if (lane == 0) { sv[warp] = bv; si[warp] = bi; }
-    __syncthreads();
-    if (warp == 0) {
-      bv = sv[lane];
-      bi = si[lane];
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-      }
-      if (lane == 0) {
-        const long long tok = sample_finish_row(s, b, bi);
-        next_tokens[b] = tok;
-        if (out_tokens) out_tokens[(size_t)b * out_stride + (*step - 1)] = tok;
-      }
-    }
-    __syncthreads();
-  }
-  if (tid == 0) {
-    if (!reset) s->steps_valid += 1;
-    if (s->eos >= 0 || s->stop2 >= 0) {
-      int all = 1;
-      for (int b = 0; b < B; ++b) all &= s->done[b];
-      s->all_done = all;
-    }
+// once every row of the step has passed sample_finish_row: count the step (count_step) and raise all_done when every row stopped
+__device__ __forceinline__ void sample_close_step(SampleState* s, int B, bool count_step) {
+  if (count_step) s->steps_valid += 1;
+  if (s->eos >= 0 || s->stop2 >= 0) {
+    const volatile int* done = s->done;             // (written by other CTAs in sample_filter_kernel)
+    int all = 1;
+    for (int b = 0; b < B; ++b) all &= done[b];
+    s->all_done = all;
   }
 }
 
-// ---- top-k / top-p (nucleus) filtering, then the Gumbel-max draw over the kept tokens ----
+// ---- stand-alone token selection: optional top-k / top-p (nucleus) filtering, then the Gumbel-max draw ----
 // For one row, with z the fp32 logits and T the temperature:
 //   s_n = z_n / T.
 //   top_k: keep n iff s_n >= the k-th largest s, duplicates counted (HF removes scores < topk(scores, k)[-1]; ties are kept).
@@ -158,11 +91,11 @@ __global__ void __launch_bounds__(1024) sample_rows_kernel(const float* __restri
 // exact k-th key by counts, then the top-p cut by w-mass among the kept keys.  Each thread accumulates 16 private bins over a
 // fixed strided subset of the row, and the bins are reduced in a fixed order; there are no floating-point atomics.  So the kept
 // set and the token are a deterministic function of (logits, T, top_k, top_p, seed, row, position).
-// One CTA per row.  The row's scores are staged in shared memory (V * 4 bytes of dynamic shared memory) when they fit;
-// otherwise every pass recomputes them from the logits in global memory.
+// One CTA per row.  With a filter, the row's scores are staged in shared memory (V * 4 bytes of dynamic shared memory) when
+// they fit; otherwise every pass recomputes them from the logits in global memory.  Without one (filter = 0) the kernel draws
+// straight from the logits (the raw logit when greedy) and is launched without dynamic shared memory.
 constexpr int kFilterThreads = 1024;
 constexpr int kFilterStageMaxBytes = 200 * 1024;     // rows of up to 51200 scores are staged
-enum { FILTER_FIRST = 0, FILTER_AFTER_MEGA = 1, FILTER_AFTER_PEROP = 2 };
 
 __device__ __forceinline__ uint32_t score_key(float s) {   // unsigned order of the keys == order of the (finite) scores
   uint32_t u = __float_as_uint(s);
@@ -171,15 +104,17 @@ __device__ __forceinline__ uint32_t score_key(float s) {   // unsigned order of 
 }
 __device__ __forceinline__ float key_score(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
 
-// mode FILTER_FIRST: the first token after a prefill (set_sampling has cleared the flags).
-// FILTER_AFTER_MEGA / FILTER_AFTER_PEROP: after a decode step that wrote `logits` and a provisional arg-max.  Overwrites
-//   next_tokens and out_tokens[:, *step - 1] and keeps done / all_done.  After the per-op kernels it also counts the step in
-//   steps_valid; the persistent kernel counts its own steps.
+// Selects the first token after a prefill (set_sampling has cleared the flags), and the token after a decode step that wrote
+// `logits` and a provisional arg-max: it then overwrites next_tokens and out_tokens[:, *step - 1].  It keeps done / all_done.
+//   per_op: after the per-op decode kernels, which step on once all_done is raised and do not count steps: a plain greedy
+//     request keeps the step's own arg-max, every row emits pad once all_done is raised, and the step is counted in
+//     steps_valid.  After the persistent kernel (which counts its own steps and skips once all_done is raised) and for the
+//     first token, none of these.
 // keep_out != nullptr (vly_test_sample_filter): writes the kept mask [B, V] and nothing else.
 __global__ void __launch_bounds__(kFilterThreads) sample_filter_kernel(const float* __restrict__ logits, int V, SampleState* s,
                                                                        const int* seq_len, const int* step, long long* next_tokens,
-                                                                       long long* out_tokens, int out_stride, int mode,
-                                                                       uint8_t* keep_out) {
+                                                                       long long* out_tokens, int out_stride, int filter,
+                                                                       int per_op, uint8_t* keep_out) {
   extern __shared__ float srow[];                   // [V] scores, when staged
   __shared__ int cnt_w[32][16];
   __shared__ float mass_w[32][16];
@@ -193,34 +128,38 @@ __global__ void __launch_bounds__(kFilterThreads) sample_filter_kernel(const flo
   __shared__ float sh_above;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, b = blockIdx.x;
   const bool select = keep_out == nullptr;
-  if (select && mode != FILTER_FIRST && s->all_done) {
-    if (mode == FILTER_AFTER_PEROP && tid == 0) {   // the per-op kernels keep stepping: emit pad, as sample_rows_kernel does
-      next_tokens[b] = s->filt.pad;
-      if (out_tokens) out_tokens[(size_t)b * out_stride + (*step - 1)] = s->filt.pad;
+  if (select && per_op && !s->enabled && s->eos < 0 && s->stop2 < 0) return;   // plain greedy: the step's arg-max is the token
+  if (select && s->all_done) {
+    if (per_op && tid == 0) {                       // the per-op kernels keep stepping: emit pad
+      next_tokens[b] = s->pad;
+      if (out_tokens) out_tokens[(size_t)b * out_stride + (*step - 1)] = s->pad;
     }
     return;                                         // (the persistent kernel skipped the step: nothing to select)
   }
-  const SampleFilter f = s->filt;
+  const float temperature = s->temperature, top_p = s->top_p;
+  const int top_k = s->top_k;
   const float* z = logits + (size_t)b * V;
-  const bool staged = (size_t)V * 4 <= (size_t)kFilterStageMaxBytes;
-  auto score = [&](int n) { return staged ? srow[n] : z[n] / f.temperature; };
+  const bool staged = filter && (size_t)V * 4 <= (size_t)kFilterStageMaxBytes;
+  auto score = [&](int n) { return staged ? srow[n] : z[n] / temperature; };
 
   uint32_t kmax = 0;
-  for (int n = tid; n < V; n += kFilterThreads) {
-    const float sc = z[n] / f.temperature;
-    if (staged) srow[n] = sc;
-    kmax = max(kmax, score_key(sc));
-  }
-  kmax = __reduce_max_sync(0xffffffffu, kmax);
-  if (lane == 0) max_w[warp] = kmax;
-  __syncthreads();
+  if (filter) {
+    for (int n = tid; n < V; n += kFilterThreads) {
+      const float sc = z[n] / temperature;
+      if (staged) srow[n] = sc;
+      kmax = max(kmax, score_key(sc));
+    }
+    kmax = __reduce_max_sync(0xffffffffu, kmax);
+    if (lane == 0) max_w[warp] = kmax;
+    __syncthreads();
 #pragma unroll 1
-  for (int w = 0; w < 32; ++w) kmax = max(kmax, max_w[w]);
+    for (int w = 0; w < 32; ++w) kmax = max(kmax, max_w[w]);
+  }
 
   uint32_t cut = 0;                                 // keep n iff score_key(s_n) >= cut
-  if (f.top_k > 0 && f.top_k < V) {
+  if (filter && top_k > 0 && top_k < V) {
     uint32_t prefix = 0, pmask = 0;
-    int krem = f.top_k;                             // rank, from the top, of the wanted key among the keys under the prefix
+    int krem = top_k;                               // rank, from the top, of the wanted key among the keys under the prefix
 #pragma unroll 1
     for (int shift = 28; shift >= 0; shift -= 4) {
       int c[16];
@@ -265,7 +204,7 @@ __global__ void __launch_bounds__(kFilterThreads) sample_filter_kernel(const flo
     cut = prefix;                                   // the k-th largest key
   }
 
-  if (f.top_p > 0.f && f.top_p < 1.f) {
+  if (filter && top_p > 0.f && top_p < 1.f) {
     const float smax = key_score(kmax);
     uint32_t prefix = 0, pmask = 0;
     float above = 0.f, target = 0.f;                // mass above the prefix's range; top_p * W (thread 0)
@@ -303,7 +242,7 @@ __global__ void __launch_bounds__(kFilterThreads) sample_filter_kernel(const flo
           if (shift == 28) {                        // every kept token is under the empty prefix: W
             float W = 0.f;
             for (int d = 15; d >= 0; --d) W += mass_d[d];
-            target = f.top_p * W;
+            target = top_p * W;
           }
           // the digit whose range holds the largest key v with (mass of the keys >= v) >= target: v is the last kept group
           float run = above;
@@ -329,55 +268,37 @@ __global__ void __launch_bounds__(kFilterThreads) sample_filter_kernel(const flo
   }
 
   const int pos = select ? *seq_len - 1 : 0;
+  const bool on = s->enabled != 0;
+  const float inv_temp = s->inv_temp;
+  const uint32_t k0 = s->seed_lo, k1 = s->seed_hi;
   float bv = -INFINITY;
   int bi = 0x7fffffff;
   for (int n = tid; n < V; n += kFilterThreads) {
-    const bool keep = score_key(score(n)) >= cut;
+    const bool keep = !filter || score_key(score(n)) >= cut;
     if (!select) {
       keep_out[(size_t)b * V + n] = keep;
     } else if (keep) {
-      const float v = sample_score(z[n], f.inv_temp, f.seed_lo, f.seed_hi, n, b, pos);
+      const float v = on ? sample_score(z[n], inv_temp, k0, k1, n, b, pos) : z[n];
       if (v > bv) { bv = v; bi = n; }               // ascending n per thread: first maximum kept
     }
   }
   if (!select) return;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-  }
+  warp_argmax(bv, bi);
   if (lane == 0) { bv_w[warp] = bv; bi_w[warp] = bi; }
   __syncthreads();
   if (warp != 0) return;
   bv = bv_w[lane];
   bi = bi_w[lane];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-  }
+  warp_argmax(bv, bi);
   if (lane != 0) return;
-  const bool stops = f.eos >= 0 || f.stop2 >= 0;
-  long long tok = bi;
-  if (stops) {                                      // sample_finish_row with the request's ids
-    if (s->done[b]) tok = f.pad;
-    else if (tok == f.eos || tok == f.stop2) s->done[b] = 1;
-  }
+  const long long tok = sample_finish_row(s, b, bi);
   next_tokens[b] = tok;
-  if (mode != FILTER_FIRST && out_tokens) out_tokens[(size_t)b * out_stride + (*step - 1)] = tok;
+  if (out_tokens) out_tokens[(size_t)b * out_stride + (*step - 1)] = tok;
   __threadfence();
-  if (atomicAdd(&s->filt_arrive, 1u) == gridDim.x - 1) {   // the last row to finish: every done flag is visible
+  if (atomicAdd(&s->arrive, 1u) == gridDim.x - 1) {   // the last row to finish: every done flag is visible
     __threadfence();
-    s->filt_arrive = 0;
-    if (mode == FILTER_AFTER_PEROP) s->steps_valid += 1;
-    if (stops) {
-      const volatile int* done = s->done;
-      int all = 1;
-      for (int r = 0; r < (int)gridDim.x; ++r) all &= done[r];
-      s->all_done = all;
-    }
+    s->arrive = 0;
+    sample_close_step(s, gridDim.x, per_op);
   }
 }
 
