@@ -14,6 +14,8 @@
 #include <memory>
 #include <mutex>
 #include <string>
+#include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "../../include/valley_b200.h"
@@ -49,7 +51,6 @@ extern "C" const char* vly_version(void) { return "valley_b200 0.1 (sm_90a)"; }
     cudaError_t e_ = (expr);                                                                           \
     if (e_ != cudaSuccess) return fail(VLY_ERR_CUDA, "%s:%d %s -> %s", __FILE__, __LINE__, #expr, cudaGetErrorString(e_)); \
   } while (0)
-#define CKL() CK(cudaGetLastError())
 #define TRY(expr)              \
   do {                         \
     int r_ = (expr);           \
@@ -149,7 +150,7 @@ struct vly_ctx {
   // workspace
   Mem w_col, w_patch, w_qkv, w_ctx, w_h, w_stats, w_pool, w_x, w_q, w_attn, w_hb, w_pstats;
   cudaStream_t cap_stream = nullptr;
-  int64_t launches = 0;
+  int64_t launches = 0;           // kernels launched (and replayed in graphs) so far: counted by launch() only
   // fused all-gather state
   Owned<bf16> g_buf;              // [g_rows, vit_hidden] + flags
   int64_t g_rows = 0;
@@ -250,7 +251,7 @@ static inline int cdiv(long long a, long long b) { return int((a + b - 1) / b); 
 static std::mutex g_attr_mu;
 static std::map<std::pair<int, const void*>, size_t> g_attr_set;
 template <typename Kern>
-static int ensure_smem_attr(int device, Kern kern, size_t bytes, bool max_carveout = false) {
+static int ensure_smem_attr(int device, Kern kern, size_t bytes, bool max_carveout) {
   std::lock_guard<std::mutex> lk(g_attr_mu);
   size_t& have = g_attr_set[std::make_pair(device, (const void*)kern)];
   if (bytes > have || (have == 0 && max_carveout)) {
@@ -291,25 +292,74 @@ static int make_tmap_3d(vly_ctx* c, CUtensorMap* m, const void* ptr, uint64_t d0
   return VLY_OK;
 }
 
-// ---- launch helper: optional programmatic dependent launch (the kernel's prologue overlaps the previous kernel's tail; kernels
-// launched this way call griddepcontrol.wait before they touch the previous kernel's data).  VLY_NO_PDL=1 disables it. ----
+// ------------------------------------------------------------------------------------------------
+// kernel launches
+// ------------------------------------------------------------------------------------------------
 static bool pdl_enabled() {
   static const bool on = getenv("VLY_NO_PDL") == nullptr;
   return on;
 }
-template <typename Kern, typename... Args>
-static cudaError_t launch_ex(Kern kern, dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, Args... args) {
+struct LaunchCfg {
+  dim3 grid, block;
+  size_t smem = 0;              // dynamic shared memory
+  cudaStream_t st = 0;
+  // programmatic dependent launch: the kernel's prologue overlaps the previous kernel's tail.  Only for kernels that call
+  // griddepcontrol.wait before they touch the previous kernel's data.  VLY_NO_PDL=1 disables it.
+  bool pdl = false;
+  bool carveout = false;        // maximum shared-memory carve-out, so the NEXT kernel's CTA can co-reside (PDL overlap)
+  bool cooperative = false;     // every CTA resident at once (grid barriers)
+};
+// Every kernel of the library is launched here, and this is the only code that counts launches (vly_kernel_launch_count;
+// capture_steps derives vly_kv::graph_nodes from the count).  cudaLaunchKernelEx converts each argument to the kernel's
+// parameter type, as <<<>>> does.
+template <typename... KArgs, typename... Args>
+static int launch(vly_ctx* c, void (*kern)(KArgs...), const LaunchCfg& l, Args&&... args) {
+  if (l.smem > 0 || l.carveout) TRY(ensure_smem_attr(c->cfg.device, kern, l.smem, l.carveout));
+  cudaLaunchAttribute attr[2];
+  unsigned n = 0;
+  if (l.pdl && pdl_enabled()) {
+    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[n++].val.programmaticStreamSerializationAllowed = 1;
+  }
+  if (l.cooperative) {
+    attr[n].id = cudaLaunchAttributeCooperative;
+    attr[n++].val.cooperative = 1;
+  }
   cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.gridDim = l.grid;
+  cfg.blockDim = l.block;
+  cfg.dynamicSmemBytes = l.smem;
+  cfg.stream = l.st;
   cfg.attrs = attr;
-  cfg.numAttrs = (pdl && pdl_enabled()) ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kern, args...);
+  cfg.numAttrs = n;
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
+  c->launches++;
+  if (e != cudaSuccess) {
+    cudaGetLastError();         // the failure is reported here; it must not surface in the caller's next error check
+    const char* name = "kernel";
+    cudaFuncGetName(&name, (const void*)kern);
+    return fail(VLY_ERR_CUDA, "launch of %s failed: %s", name, cudaGetErrorString(e));
+  }
+  return VLY_OK;
+}
+
+// The decode kernels are compiled for 1, 2 or 4 batch rows: f(std::integral_constant<int, rows for B>).
+static inline int bmax_of(int B) { return B <= 1 ? 1 : (B <= 2 ? 2 : 4); }
+template <typename F>
+static int with_bmax(int B, F&& f) {
+  if (bmax_of(B) == 1) return f(std::integral_constant<int, 1>());
+  if (bmax_of(B) == 2) return f(std::integral_constant<int, 2>());
+  return f(std::integral_constant<int, 4>());
+}
+// VLY_F32 / VLY_BF16 / VLY_F16 -> f(Type<float | bf16 | __half>)
+template <typename T>
+struct Type { using type = T; };
+template <typename F>
+static int with_dtype(int dtype, F&& f) {
+  if (dtype == VLY_F32) return f(Type<float>());
+  if (dtype == VLY_BF16) return f(Type<bf16>());
+  if (dtype == VLY_F16) return f(Type<__half>());
+  return fail(VLY_ERR_INVALID, "unknown dtype %d", dtype);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -324,10 +374,7 @@ static int launch_gemm_t(vly_ctx* c, const bf16* A, long long lda, const bf16* W
   p.num_m_tiles = cdiv(p.M, 128);
   p.num_n_tiles = cdiv(p.N, BN);
   const int tiles = p.num_m_tiles * p.num_n_tiles;
-  TRY(ensure_smem_attr(c->cfg.device, gemm_tc_kernel<BN, EPI>, Cfg::SMEM_BYTES));
-  CK(launch_ex(gemm_tc_kernel<BN, EPI>, dim3(tiles), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, true, ta, tb, p));
-  c->launches++;
-  return VLY_OK;
+  return launch(c, gemm_tc_kernel<BN, EPI>, {dim3(tiles), dim3(Cfg::THREADS), Cfg::SMEM_BYTES, st, true}, ta, tb, p);
 }
 template <int EPI>
 static int launch_gemm(vly_ctx* c, int bn, const bf16* A, long long lda, const bf16* W, long long ldw, const GemmParams& p,
@@ -484,6 +531,7 @@ extern "C" int vly_num_sms(vly_ctx* c, int* out) {
 }
 extern "C" int vly_kernel_launch_count(vly_ctx* c, int64_t* out) {
   if (!c || !out) return fail(VLY_ERR_INVALID, "null");
+  std::lock_guard<std::mutex> lk(c->mu);
   *out = c->launches;
   return VLY_OK;
 }
@@ -519,17 +567,17 @@ extern "C" int vly_load_weight(vly_ctx* c, const char* name, const void* dev_ptr
   s.is_f32 = (ndim == 1) || ends_with(nm, "position_embedding.weight");
   c->staged.erase(nm);
   TRY(s.mem.alloc((size_t)s.numel * (s.is_f32 ? 4 : 2)));
-  const int blocks = (int)std::min<long long>((s.numel + 255) / 256, 4096);
-  if (s.is_f32) {
-    if (dtype == VLY_F32) convert_to_f32_bf16rounded_kernel<float><<<blocks, 256>>>((const float*)dev_ptr, (float*)s.mem.p, s.numel);
-    else if (dtype == VLY_BF16) convert_to_f32_bf16rounded_kernel<bf16><<<blocks, 256>>>((const bf16*)dev_ptr, (float*)s.mem.p, s.numel);
-    else convert_to_f32_bf16rounded_kernel<__half><<<blocks, 256>>>((const __half*)dev_ptr, (float*)s.mem.p, s.numel);
-  } else {
-    if (dtype == VLY_F32) convert_to_bf16_kernel<float><<<blocks, 256>>>((const float*)dev_ptr, (bf16*)s.mem.p, s.numel);
-    else if (dtype == VLY_BF16) CK(cudaMemcpyAsync(s.mem.p, dev_ptr, (size_t)s.numel * 2, cudaMemcpyDeviceToDevice, 0));
-    else convert_to_bf16_kernel<__half><<<blocks, 256>>>((const __half*)dev_ptr, (bf16*)s.mem.p, s.numel);
-  }
-  CKL();
+  const LaunchCfg l = {dim3((unsigned)std::min<long long>((s.numel + 255) / 256, 4096)), dim3(256)};
+  TRY(with_dtype(dtype, [&](auto t) -> int {
+    using E = typename decltype(t)::type;
+    if (s.is_f32) return launch(c, convert_to_f32_bf16rounded_kernel<E>, l, (const E*)dev_ptr, (float*)s.mem.p, s.numel);
+    if constexpr (std::is_same<E, bf16>::value) {         // a bf16 matrix is already in its staged format
+      CK(cudaMemcpyAsync(s.mem.p, dev_ptr, (size_t)s.numel * 2, cudaMemcpyDeviceToDevice, 0));
+      return VLY_OK;
+    } else {
+      return launch(c, convert_to_bf16_kernel<E>, l, (const E*)dev_ptr, (bf16*)s.mem.p, s.numel);
+    }
+  }));
   CK(cudaStreamSynchronize(0));  // the caller may free its tensor right after we return
   c->staged[nm] = std::move(s);
   return VLY_OK;
@@ -577,8 +625,8 @@ extern "C" int vly_finalize_weights(vly_ctx* c) {
     TRY(take(c, vp + "pre_layrnorm.weight", true, D, &c->pre_g));
     TRY(take(c, vp + "pre_layrnorm.bias", true, D, &c->pre_b));
     TRY(c->patch_w.alloc((size_t)D * c->kpad * 2));
-    pack_rows_kernel<<<D, 256>>>((bf16*)pw, KK, nullptr, nullptr, nullptr, c->patch_w, c->kpad, 0, 0, nullptr, nullptr);
-    CKL();
+    TRY(launch(c, pack_rows_kernel, {dim3(D), dim3(256)}, (bf16*)pw, KK, nullptr, nullptr, nullptr, c->patch_w, c->kpad, 0, 0, nullptr,
+               nullptr));
     CK(cudaDeviceSynchronize());
     drop_staged(c, vp + "embeddings.patch_embedding.weight");
     c->vit.resize(g.vit_layers);
@@ -598,8 +646,8 @@ extern "C" int vly_finalize_weights(vly_ctx* c) {
         void *ww, *bb;
         TRY(get_staged(c, q + "self_attn." + nm[i] + ".weight", false, (int64_t)D * D, &ww));
         TRY(get_staged(c, q + "self_attn." + nm[i] + ".bias", true, D, &bb));
-        pack_rows_kernel<<<D, 256>>>((bf16*)ww, D, (float*)g1, (float*)b1n, (float*)bb, w.wqkv, D, 0, i * D, w.qkv_cs, w.qkv_b);
-        CKL();
+        TRY(launch(c, pack_rows_kernel, {dim3(D), dim3(256)}, (bf16*)ww, D, (float*)g1, (float*)b1n, (float*)bb, w.wqkv, D, 0, i * D,
+                   w.qkv_cs, w.qkv_b));
         CK(cudaDeviceSynchronize());
         drop_staged(c, q + "self_attn." + nm[i] + ".weight");
       }
@@ -613,8 +661,7 @@ extern "C" int vly_finalize_weights(vly_ctx* c) {
       TRY(w.w1.alloc((size_t)M * D * 2));
       TRY(w.c1.alloc(M * 4));
       TRY(w.b1.alloc(M * 4));
-      pack_rows_kernel<<<M, 256>>>((bf16*)w1, D, (float*)g2, (float*)b2n, (float*)b1, w.w1, D, 0, 0, w.c1, w.b1);
-      CKL();
+      TRY(launch(c, pack_rows_kernel, {dim3(M), dim3(256)}, (bf16*)w1, D, (float*)g2, (float*)b2n, (float*)b1, w.w1, D, 0, 0, w.c1, w.b1));
       CK(cudaDeviceSynchronize());
       drop_staged(c, q + "mlp.fc1.weight");
     }
@@ -626,8 +673,7 @@ extern "C" int vly_finalize_weights(vly_ctx* c) {
         void* pw;
         TRY(get_staged(c, "model.pooling_layer.weight", false, (int64_t)NP * H, &pw));
         TRY(c->pool_U.alloc((size_t)NP * D * 4));
-        fold_importance_kernel<<<NP, 256>>>((const bf16*)pw, c->proj_w, c->pool_U, H, D);      // the bias cancels in the softmax
-        CKL();
+        TRY(launch(c, fold_importance_kernel, {dim3(NP), dim3(256)}, (const bf16*)pw, c->proj_w, c->pool_U, H, D));  // the bias cancels in the softmax
         CK(cudaDeviceSynchronize());
         drop_staged(c, "model.pooling_layer.weight");
       } else if (g.patch_pooling_method == VLY_POOL_TEMPORAL_TRANSFORMER) {   // valley_model.py:45-52
@@ -667,8 +713,8 @@ extern "C" int vly_finalize_weights(vly_ctx* c) {
       for (int i = 0; i < 3; ++i) {
         void* ww;
         TRY(get_staged(c, q + "self_attn." + nm[i] + ".weight", false, (int64_t)H * H, &ww));
-        pack_rows_kernel<<<H, 256>>>((bf16*)ww, H, (float*)g1, nullptr, nullptr, w.wqkv, H, i < 2 ? 1 : 0, i * H, nullptr, nullptr);
-        CKL();
+        TRY(launch(c, pack_rows_kernel, {dim3(H), dim3(256)}, (bf16*)ww, H, (float*)g1, nullptr, nullptr, w.wqkv, H, i < 2 ? 1 : 0, i * H,
+                   nullptr, nullptr));
         CK(cudaDeviceSynchronize());
         drop_staged(c, q + "self_attn." + nm[i] + ".weight");
       }
@@ -678,9 +724,8 @@ extern "C" int vly_finalize_weights(vly_ctx* c) {
       TRY(get_staged(c, q + "mlp.up_proj.weight", false, (int64_t)I * H, &wu));
       TRY(take(c, q + "mlp.down_proj.weight", false, (int64_t)H * I, &w.wdown));
       TRY(w.wgu.alloc((size_t)2 * I * H * 2));
-      pack_rows_kernel<<<I, 256>>>((bf16*)wg, H, (float*)g2, nullptr, nullptr, w.wgu, H, 2, 0, nullptr, nullptr);
-      pack_rows_kernel<<<I, 256>>>((bf16*)wu, H, (float*)g2, nullptr, nullptr, w.wgu, H, 2, 1, nullptr, nullptr);
-      CKL();
+      TRY(launch(c, pack_rows_kernel, {dim3(I), dim3(256)}, (bf16*)wg, H, (float*)g2, nullptr, nullptr, w.wgu, H, 2, 0, nullptr, nullptr));
+      TRY(launch(c, pack_rows_kernel, {dim3(I), dim3(256)}, (bf16*)wu, H, (float*)g2, nullptr, nullptr, w.wgu, H, 2, 1, nullptr, nullptr));
       CK(cudaDeviceSynchronize());
       drop_staged(c, q + "mlp.gate_proj.weight");
       drop_staged(c, q + "mlp.up_proj.weight");
@@ -689,13 +734,12 @@ extern "C" int vly_finalize_weights(vly_ctx* c) {
     TRY(get_staged(c, "model.norm.weight", true, H, &nf));
     TRY(get_staged(c, "lm_head.weight", false, (int64_t)V * H, &lm));
     TRY(c->lm_head.alloc((size_t)V * H * 2));
-    pack_rows_kernel<<<V, 256>>>((bf16*)lm, H, (float*)nf, nullptr, nullptr, c->lm_head, H, 0, 0, nullptr, nullptr);
-    CKL();
+    TRY(launch(c, pack_rows_kernel, {dim3(V), dim3(256)}, (bf16*)lm, H, (float*)nf, nullptr, nullptr, c->lm_head, H, 0, 0, nullptr, nullptr));
     CK(cudaDeviceSynchronize());
     drop_staged(c, "lm_head.weight");
     TRY(c->rope.alloc((size_t)g.max_position_embeddings * 64 * sizeof(float2)));
-    rope_table_kernel<<<cdiv((long long)g.max_position_embeddings * 64, 256), 256>>>(c->rope, g.max_position_embeddings, g.rope_theta, 128);
-    CKL();
+    TRY(launch(c, rope_table_kernel, {dim3(cdiv((long long)g.max_position_embeddings * 64, 256)), dim3(256)}, c->rope,
+               g.max_position_embeddings, g.rope_theta, 128));
   }
   CK(cudaDeviceSynchronize());
   c->staged.clear();
@@ -710,7 +754,6 @@ static int launch_vit_attention(vly_ctx* c, const bf16* qkv, int F, bf16* out, c
   const vly_config& g = c->cfg;
   const int D = g.vit_hidden, tokens = (g.vit_image / g.vit_patch) * (g.vit_image / g.vit_patch) + 1;
   using C = FlashCfg<64>;
-  TRY(ensure_smem_attr(c->cfg.device, vit_attention_kernel, C::SMEM_BYTES));
   CUtensorMap tq;
   TRY(make_tmap_2d(c, &tq, qkv, 3 * D, (uint64_t)F * tokens, (uint64_t)3 * D * 2, 64, 64));
   VitAttnParams p;
@@ -721,9 +764,7 @@ static int launch_vit_attention(vly_ctx* c, const bf16* qkv, int F, bf16* out, c
   p.ctx = out;
   p.scale_log2e = 0.125f * 1.4426950408889634f;
   const int grid = F * g.vit_heads * cdiv(tokens, 64);
-  CK(launch_ex(vit_attention_kernel, dim3(grid), dim3(C::THREADS), C::SMEM_BYTES, st, true, tq, p));
-  c->launches++;
-  return VLY_OK;
+  return launch(c, vit_attention_kernel, {dim3(grid), dim3(C::THREADS), C::SMEM_BYTES, st, true}, tq, p);
 }
 
 static int vit_layers_needed(const vly_config& g, int select_layer, int* out) {
@@ -752,6 +793,8 @@ static int vit_encode_impl(vly_ctx* c, const void* pixels, int pixel_dtype, int 
   const int NP = (IMG / P) * (IMG / P), tokens = NP + 1;
   int n_layers;
   TRY(vit_layers_needed(g, select_layer, &n_layers));
+  if (pixel_dtype != VLY_F32 && pixel_dtype != VLY_BF16 && pixel_dtype != VLY_F16)
+    return fail(VLY_ERR_INVALID, "vly_vit_encode: unknown pixel dtype %d", pixel_dtype);
   const int CH = 256;  // frames per chunk: bounds the workspace (qkv 405 MB, mlp 540 MB) and keeps tiles plentiful
   const int fc_max = F < CH ? F : CH;
   const size_t Mmax = (size_t)fc_max * tokens;
@@ -770,13 +813,10 @@ static int vit_encode_impl(vly_ctx* c, const void* pixels, int pixel_dtype, int 
     const char* px = (const char*)pixels + (size_t)f0 * 3 * IMG * IMG * px_elem;
     bf16* x = (bf16*)out_dev + (size_t)f0 * tokens * D;
     bf16* col = (bf16*)c->w_col.p;
-    const int blocks = c->num_sms * 8;
-    if (pixel_dtype == VLY_F32) im2col_kernel<float><<<blocks, 256, 0, st>>>((const float*)px, col, fc, IMG, P, c->kpad);
-    else if (pixel_dtype == VLY_BF16) im2col_kernel<bf16><<<blocks, 256, 0, st>>>((const bf16*)px, col, fc, IMG, P, c->kpad);
-    else if (pixel_dtype == VLY_F16) im2col_kernel<__half><<<blocks, 256, 0, st>>>((const __half*)px, col, fc, IMG, P, c->kpad);
-    else return fail(VLY_ERR_INVALID, "vly_vit_encode: unknown pixel dtype %d", pixel_dtype);
-    c->launches++;
-    CKL();
+    TRY(with_dtype(pixel_dtype, [&](auto t) {
+      using E = typename decltype(t)::type;
+      return launch(c, im2col_kernel<E>, {dim3(c->num_sms * 8), dim3(256), 0, st}, (const E*)px, col, fc, IMG, P, c->kpad);
+    }));
     {  // patch embedding GEMM (conv2d stride=kernel=14, no bias)
       GemmParams p = {};
       p.M = fc * NP; p.N = D; p.K = c->kpad;
@@ -784,9 +824,8 @@ static int vit_encode_impl(vly_ctx* c, const void* pixels, int pixel_dtype, int 
       TRY(launch_gemm<EPI_BIAS>(c, pick_bn_m(c, D, fc * NP), col, c->kpad, c->patch_w, c->kpad, p, st));
     }
     float2* stats = (float2*)c->w_stats.p;
-    vit_embed_ln_kernel<<<M, 128, 0, st>>>((bf16*)c->w_patch.p, c->cls, c->pos, c->pre_g, c->pre_b, x, stats, nt, tokens, D, g.vit_eps);
-    c->launches++;
-    CKL();
+    TRY(launch(c, vit_embed_ln_kernel, {dim3(M), dim3(128), 0, st}, (bf16*)c->w_patch.p, c->cls, c->pos, c->pre_g, c->pre_b, x, stats, nt,
+               tokens, D, g.vit_eps));
     for (int l = 0; l < n_layers; ++l) {
       const VitLayerW& w = c->vit[l];
       {  // LN1 -> q,k,v
@@ -922,10 +961,7 @@ extern "C" int vly_gather_release(vly_ctx* c, void* stream) {
   CK(cudaSetDevice(c->cfg.device));
   PeerFlags pf;
   for (int q = 0; q < 8; ++q) pf.p[q] = c->g_peer_flags[q] ? c->g_peer_flags[q] + 8 : nullptr;
-  gather_signal_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(pf, c->g_world, c->g_rank, c->g_epoch);
-  c->launches++;
-  CKL();
-  return VLY_OK;
+  return launch(c, gather_signal_kernel, {dim3(1), dim3(32), 0, (cudaStream_t)stream}, pf, c->g_world, c->g_rank, c->g_epoch);
 }
 
 extern "C" int vly_vit_encode_gather(vly_ctx* c, const void* pixels, int pixel_dtype, int F, int frame_offset, int select_layer, void* stream) {
@@ -946,9 +982,7 @@ extern "C" int vly_vit_encode_gather_strided(vly_ctx* c, const void* pixels, int
   TRY(gather_check_timeout(c, "vly_vit_encode_gather"));
   int* timeout_flag = c->g_timeout;
   if (c->g_epoch > 0) {   // every rank must have finished READING the previous epoch before anyone overwrites its buffer
-    gather_wait_kernel<<<1, 32, 0, st>>>(c->g_flags + 8, c->g_world, c->g_epoch, timeout_flag);
-    c->launches++;
-    CKL();
+    TRY(launch(c, gather_wait_kernel, {dim3(1), dim3(32), 0, st}, c->g_flags + 8, c->g_world, c->g_epoch, timeout_flag));
   }
   if (F > 0) {
     TRY(ensure(c->w_xlocal, (size_t)F * tokens * c->cfg.vit_hidden * 2));       // local residual stream (scratch)
@@ -958,11 +992,8 @@ extern "C" int vly_vit_encode_gather_strided(vly_ctx* c, const void* pixels, int
   const int epoch = ++c->g_epoch;
   PeerFlags pf;
   for (int q = 0; q < 8; ++q) pf.p[q] = c->g_peer_flags[q];
-  gather_signal_kernel<<<1, 32, 0, st>>>(pf, c->g_world, c->g_rank, epoch);
-  gather_wait_kernel<<<1, 32, 0, st>>>(c->g_flags, c->g_world, epoch, timeout_flag);
-  c->launches += 2;
-  CKL();
-  return VLY_OK;
+  TRY(launch(c, gather_signal_kernel, {dim3(1), dim3(32), 0, st}, pf, c->g_world, c->g_rank, epoch));
+  return launch(c, gather_wait_kernel, {dim3(1), dim3(32), 0, st}, c->g_flags, c->g_world, epoch, timeout_flag);
 }
 
 extern "C" int vly_project(vly_ctx* c, const void* feats, int64_t rows, void* out, void* stream) {
@@ -1007,42 +1038,35 @@ static int pool_project_after(vly_ctx* c, const bf16* feats, int n_videos, int T
       p.M = T * tokens; p.N = H; p.K = D; p.out = P; p.ldo = H; p.bias = c->proj_b;
       TRY(launch_gemm<EPI_BIAS>(c, pick_bn_m(c, H, p.M), feats + (size_t)v * T * tokens * D, D, c->proj_w, D, p, st));
     }
+    const LaunchCfg two_per_sm = {dim3(c->num_sms * 2), dim3(256), 0, st};
     if (!tr) {
-      temporal_max_kernel<<<c->num_sms * 2, 256, 0, st>>>(P, vis, T, tokens, H);
-      c->launches++;
-      CKL();
+      TRY(launch(c, temporal_max_kernel, two_per_sm, P, vis, T, tokens, H));
       continue;
     }
     bf16 *Xp = (bf16*)c->w_xp.p, *KV = (bf16*)c->w_dkv.p, *Q = (bf16*)c->w_dq.p, *att = (bf16*)c->w_datt.p;
     bf16 *X1 = (bf16*)c->w_dx1.p, *F1 = (bf16*)c->w_df1.p, *X2 = (bf16*)c->w_dx2.p;
     const bf16* Xlast = Xp + (size_t)(T - 1) * NP * H;          // rows of the last frame: the only queries that are used (:130)
-    delta_add_pos_kernel<<<c->num_sms * 2, 256, 0, st>>>(P, w.pos, Xp, T, tokens, H);
-    c->launches++;
+    TRY(launch(c, delta_add_pos_kernel, two_per_sm, P, w.pos, Xp, T, tokens, H));
     GemmParams p = {};
     p.M = T * NP; p.N = 2 * H; p.K = H; p.out = KV; p.ldo = 2 * H; p.bias = w.in_b + H;          // k | v rows of in_proj
     TRY(launch_gemm<EPI_BIAS>(c, pick_bn_m(c, p.N, p.M), Xp, H, w.in_w + (size_t)H * H, H, p, st));
     p = {};
     p.M = NP; p.N = H; p.K = H; p.out = Q; p.ldo = H; p.bias = w.in_b;
     TRY(launch_gemm<EPI_BIAS>(c, pick_bn_m(c, p.N, p.M), Xlast, H, w.in_w, H, p, st));
-    delta_attention_kernel<<<NP, nhead * 32, 0, st>>>(Q, KV, att, T, NP, H, nhead);
-    c->launches++;
+    TRY(launch(c, delta_attention_kernel, {dim3(NP), dim3(nhead * 32), 0, st}, Q, KV, att, T, NP, H, nhead));
     p = {};
     p.M = NP; p.N = H; p.K = H; p.out = X1; p.ldo = H; p.bias = w.out_b; p.residual = Xlast; p.ldr = H;
     TRY(launch_gemm<EPI_BIAS_RES_STATS>(c, pick_bn_m(c, p.N, p.M), att, H, w.out_w, H, p, st));
-    layernorm_rows_kernel<<<NP, 256, 0, st>>>(X1, w.n1_g, w.n1_b, X1, H, 1e-5f);
-    c->launches++;
+    TRY(launch(c, layernorm_rows_kernel, {dim3(NP), dim3(256), 0, st}, X1, w.n1_g, w.n1_b, X1, H, 1e-5f));
     p = {};
     p.M = NP; p.N = w.ffn; p.K = H; p.out = F1; p.ldo = w.ffn; p.bias = w.l1_b;
     TRY(launch_gemm<EPI_BIAS>(c, pick_bn_m(c, p.N, p.M), X1, H, w.l1_w, H, p, st));
-    relu_inplace_kernel<<<c->num_sms, 256, 0, st>>>(F1, (long long)NP * w.ffn / 8);
-    c->launches++;
+    TRY(launch(c, relu_inplace_kernel, {dim3(c->num_sms), dim3(256), 0, st}, F1, (long long)NP * w.ffn / 8));
     p = {};
     p.M = NP; p.N = H; p.K = w.ffn; p.out = X2; p.ldo = H; p.bias = w.l2_b; p.residual = X1; p.ldr = H;
     TRY(launch_gemm<EPI_BIAS_RES_STATS>(c, pick_bn_m(c, p.N, p.M), F1, w.ffn, w.l2_w, w.ffn, p, st));
-    layernorm_rows_kernel<<<NP, 256, 0, st>>>(X2, w.n2_g, w.n2_b, X2, H, 1e-5f);
-    delta_finish_kernel<<<c->num_sms * 2, 256, 0, st>>>(P, X2, vis, T, tokens, H);
-    c->launches += 2;
-    CKL();
+    TRY(launch(c, layernorm_rows_kernel, {dim3(NP), dim3(256), 0, st}, X2, w.n2_g, w.n2_b, X2, H, 1e-5f));
+    TRY(launch(c, delta_finish_kernel, two_per_sm, P, X2, vis, T, tokens, H));
   }
   return VLY_OK;
 }
@@ -1063,14 +1087,14 @@ extern "C" int vly_pool_project(vly_ctx* c, const void* feats, int n_videos, int
     // softmax_t(w . flatten(proj(x_t))) weights: scores straight from the ViT features through the folded U (pooling_kernels.cuh)
     if (!c->pool_U) return fail(VLY_ERR_STATE, "vly_pool_project: model.pooling_layer.weight not loaded");
     TRY(ensure(c->w_score, (size_t)n_videos * T * 4));
-    importance_score_kernel<<<dim3(T, n_videos), 256, 0, st>>>((const bf16*)feats, c->pool_U, (float*)c->w_score.p, T, tokens, D);
-    weighted_pool_kernel<<<c->num_sms * 4, 256, 0, st>>>((const bf16*)feats, (const float*)c->w_score.p, (bf16*)c->w_pool.p, n_videos, T, tokens, D);
-    c->launches++;
+    TRY(launch(c, importance_score_kernel, {dim3(T, n_videos), dim3(256), 0, st}, (const bf16*)feats, c->pool_U, (float*)c->w_score.p, T,
+               tokens, D));
+    TRY(launch(c, weighted_pool_kernel, {dim3(c->num_sms * 4), dim3(256), 0, st}, (const bf16*)feats, (const float*)c->w_score.p,
+               (bf16*)c->w_pool.p, n_videos, T, tokens, D));
   } else {
-    temporal_pool_kernel<<<c->num_sms * 4, 256, 0, st>>>((const bf16*)feats, (bf16*)c->w_pool.p, n_videos, T, tokens, D);
+    TRY(launch(c, temporal_pool_kernel, {dim3(c->num_sms * 4), dim3(256), 0, st}, (const bf16*)feats, (bf16*)c->w_pool.p, n_videos, T,
+               tokens, D));
   }
-  c->launches++;
-  CKL();
   GemmParams p = {};
   p.M = n_videos * rows; p.N = g.hidden_size; p.K = D;
   p.out = vis_rows; p.ldo = g.hidden_size; p.bias = c->proj_b;
@@ -1084,11 +1108,8 @@ extern "C" int vly_embed_splice(vly_ctx* c, const int64_t* ids, const int32_t* s
   std::lock_guard<std::mutex> lk(c->mu);
   if (!c->finalized || !c->has_llm) return fail(VLY_ERR_STATE, "vly_embed_splice: LLM weights not loaded");
   CK(cudaSetDevice(c->cfg.device));
-  embed_splice_kernel<<<B * S, 128, 0, (cudaStream_t)stream>>>((const long long*)ids, src_map, img_idx, c->embed, (const bf16*)vis_rows,
-                                                               rows_per_img, (bf16*)out, nullptr, 0, S, c->cfg.hidden_size, c->cfg.vocab_size);
-  c->launches++;
-  CKL();
-  return VLY_OK;
+  return launch(c, embed_splice_kernel, {dim3(B * S), dim3(128), 0, (cudaStream_t)stream}, (const long long*)ids, src_map, img_idx, c->embed,
+                (const bf16*)vis_rows, rows_per_img, (bf16*)out, nullptr, 0, S, c->cfg.hidden_size, c->cfg.vocab_size);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1185,7 +1206,7 @@ static void pick_phase_geometry(const DecodeSettings& s, int bmax, size_t ring_b
 static int plan_decode_mega(vly_ctx* c, vly_kv* kv, const DecodeSettings& s) {
   const vly_config& g = c->cfg;
   const int B = kv->B, H = g.hidden_size, nH = g.num_attention_heads, I = g.intermediate_size, V = g.vocab_size;
-  const int bmax = B <= 1 ? 1 : (B <= 2 ? 2 : 4);
+  const int bmax = bmax_of(B);
   const int pad = bmax > 1 ? MegaCfg::PAD_TC : 0;
   size_t x_bytes, misc;
   mega_smem_layout(g, bmax, &x_bytes, &misc);
@@ -1328,8 +1349,7 @@ extern "C" int vly_kv_create(vly_ctx* c, int batch, int max_seq, vly_kv** out) {
 
 extern "C" int vly_kv_decode_kernel(vly_kv* kv, char* name, int cap) {
   if (!kv || !name || cap <= 0) return fail(VLY_ERR_INVALID, "vly_kv_decode_kernel: bad argument");
-  const int bmax = kv->B <= 1 ? 1 : (kv->B <= 2 ? 2 : 4);
-  if (kv->B <= 4) snprintf(name, (size_t)cap, "decode_step_kernel<%d>", bmax);
+  if (kv->B <= 4) snprintf(name, (size_t)cap, "decode_step_kernel<%d>", bmax_of(kv->B));
   else snprintf(name, (size_t)cap, "per-op TMA-ring decode kernels");
   return VLY_OK;
 }
@@ -1382,23 +1402,21 @@ extern "C" int vly_kv_set_key_mask(vly_kv* kv, const uint8_t* mask_dev, int len,
     kv->masked = false;
     return VLY_OK;
   }
-  pack_key_mask_kernel<<<dim3(cdiv(words, 128), kv->B), 128, 0, (cudaStream_t)stream>>>(mask_dev, len, words, kv->key_bits);
-  kv->ctx->launches++;
-  CKL();
+  TRY(launch(kv->ctx, pack_key_mask_kernel, {dim3(cdiv(words, 128), kv->B), dim3(128), 0, (cudaStream_t)stream}, mask_dev, len, words,
+             kv->key_bits));
   kv->masked = true;
   return VLY_OK;
 }
 
 extern "C" int vly_kv_export(vly_ctx* c, vly_kv* kv, int layer, int which, void* out, void* stream) {
   if (!c || !kv || !out || layer < 0 || layer >= c->cfg.num_hidden_layers || (which != 0 && which != 1)) return fail(VLY_ERR_INVALID, "vly_kv_export: bad argument");
-  TRY(sync_len(kv));
+  if (kv->ctx != c) return fail(VLY_ERR_INVALID, "vly_kv_export: the kv cache belongs to another context");
+  TRY(sync_len(kv));     // (before the lock: it waits on this cache's last generate only)
   if (kv->host_len == 0) return VLY_OK;
+  std::lock_guard<std::mutex> lk(c->mu);
   CK(cudaSetDevice(c->cfg.device));
-  dim3 grid(kv->host_len, kv->B * c->cfg.num_attention_heads);
-  kv_export_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(which ? kv->v_layer(layer) : kv->k_layer(layer), (bf16*)out, kv->Smax, kv->host_len, which == 0);
-  c->launches++;
-  CKL();
-  return VLY_OK;
+  return launch(c, kv_export_kernel, {dim3(kv->host_len, kv->B * c->cfg.num_attention_heads), dim3(128), 0, (cudaStream_t)stream},
+                which ? kv->v_layer(layer) : kv->k_layer(layer), (bf16*)out, kv->Smax, kv->host_len, which == 0);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1407,7 +1425,7 @@ extern "C" int vly_kv_export(vly_ctx* c, vly_kv* kv, int layer, int which, void*
 // ---- per-op decode launchers (TMA ring + programmatic dependent launch) ----
 template <int MODE>
 static int launch_gemv_ring(vly_ctx* c, GemvParams p, bool pdl, cudaStream_t st) {
-  const int bmax = p.B <= 1 ? 1 : (p.B <= 2 ? 2 : 4);
+  const int bmax = bmax_of(p.B);
   if (p.B > 4) return fail(VLY_ERR_INVALID, "gemv: batch %d > 4 per call (callers split the batch)", p.B);
   if (p.ldx == 0) p.ldx = p.K;
   const size_t x_bytes = (((size_t)bmax * p.K * 2) + 15) & ~size_t(15);
@@ -1421,21 +1439,8 @@ static int launch_gemv_ring(vly_ctx* c, GemvParams p, bool pdl, cudaStream_t st)
   }
   const size_t smem = (size_t)n_stages * RingCfg::STAGE_BYTES + x_bytes + misc;
   const int groups = (p.N + RingCfg::ROWS - 1) / RingCfg::ROWS;
-  const int grid = groups < c->num_sms ? groups : c->num_sms;
-  cudaError_t e;
-#define VLY_RING_CASE(BM)                                                                                                   \
-  {                                                                                                                         \
-    /* maximum shared-memory carve-out so the NEXT kernel's CTA can co-reside (PDL overlap) */                            \
-    TRY(ensure_smem_attr(c->cfg.device, gemv_ring_kernel<BM, MODE>, smem, true));                                           \
-    e = launch_ex(gemv_ring_kernel<BM, MODE>, dim3(grid), dim3(RingCfg::THREADS), smem, st, pdl, p, n_stages);              \
-  }
-  if (bmax == 1) VLY_RING_CASE(1)
-  else if (bmax == 2) VLY_RING_CASE(2)
-  else VLY_RING_CASE(4)
-#undef VLY_RING_CASE
-  c->launches++;
-  CK(e);
-  return VLY_OK;
+  const LaunchCfg l = {dim3(groups < c->num_sms ? groups : c->num_sms), dim3(RingCfg::THREADS), smem, st, pdl, true};
+  return with_bmax(p.B, [&](auto bm) { return launch(c, gemv_ring_kernel<decltype(bm)::value, MODE>, l, p, n_stages); });
 }
 
 // Enqueue one decode step for batch rows [b0, b0+nb) of kv (nb <= 4).  Reads kv->cur_tokens, writes kv->cur_tokens.
@@ -1443,9 +1448,7 @@ static int enqueue_decode_step(vly_ctx* c, vly_kv* kv, int b0, int nb, bool bump
   const vly_config& g = c->cfg;
   const int H = g.hidden_size, nH = g.num_attention_heads, I = g.intermediate_size, V = g.vocab_size;
   bf16 *x = kv->x + (size_t)b0 * H, *q = kv->q + (size_t)b0 * H, *attn = kv->attn + (size_t)b0 * H, *hb = kv->hb + (size_t)b0 * I;
-  decode_embed_kernel<<<nb, 256, 0, st>>>(kv->cur_tokens + b0, c->embed, x, H, V);
-  c->launches++;
-  CKL();
+  TRY(launch(c, decode_embed_kernel, {dim3(nb), dim3(256), 0, st}, kv->cur_tokens + b0, c->embed, x, H, V));
   for (int l = 0; l < g.num_hidden_layers; ++l) {
     const LlamaLayerW& w = c->layers[l];
     bf16* kc = kv->k_layer(l) + (size_t)b0 * nH * kv->Smax * 128;
@@ -1467,10 +1470,7 @@ static int enqueue_decode_step(vly_ctx* c, vly_kv* kv, int b0, int nb, bool bump
       p.out = attn;
       p.scale_log2e = 0.08838834764831845f * 1.4426950408889634f;
       p.key_bits = kv->key_bits + (size_t)b0 * kv->mask_words(); p.mask_words = kv->mask_words();
-      TRY(ensure_smem_attr(c->cfg.device, decode_attention_v2_kernel, 0, true));
-      dim3 grid(nb * nH, p.nsplit);
-      CK(launch_ex(decode_attention_v2_kernel, grid, dim3(128), 0, st, true, p));
-      c->launches++;
+      TRY(launch(c, decode_attention_v2_kernel, {dim3(nb * nH, p.nsplit), dim3(128), 0, st, true, true}, p));
     }
     {
       GemvParams p = {};
@@ -1513,7 +1513,6 @@ static int launch_prefill_attention(vly_ctx* c, vly_kv* kv, const bf16* qbuf, in
   const vly_config& g = c->cfg;
   const int H = g.hidden_size, nH = g.num_attention_heads;
   using C = FlashCfg<128>;
-  TRY(ensure_smem_attr(c->cfg.device, llama_prefill_attention_kernel, C::SMEM_BYTES));
   CUtensorMap tq, tk, tv;
   TRY(make_tmap_2d(c, &tq, qbuf, H, (uint64_t)B * S, (uint64_t)H * 2, 64, 64));
   TRY(make_tmap_3d(c, &tk, kv->k_layer(layer), 128, kv->Smax, (uint64_t)B * nH, 256, (uint64_t)kv->Smax * 256, 64, 64));
@@ -1523,9 +1522,7 @@ static int launch_prefill_attention(vly_ctx* c, vly_kv* kv, const bf16* qbuf, in
   p.scale_log2e = 0.08838834764831845f * 1.4426950408889634f;
   p.key_bits = kv->masked ? static_cast<uint32_t*>(kv->key_bits) : nullptr; p.mask_words = kv->mask_words();
   const int n_qt = cdiv(S, 64);
-  CK(launch_ex(llama_prefill_attention_kernel, dim3(B * nH * n_qt), dim3(C::THREADS), C::SMEM_BYTES, st, true, tq, tk, tv, p));
-  c->launches++;
-  return VLY_OK;
+  return launch(c, llama_prefill_attention_kernel, {dim3(B * nH * n_qt), dim3(C::THREADS), C::SMEM_BYTES, st, true}, tq, tk, tv, p);
 }
 
 extern "C" int vly_llama_prefill(vly_ctx* c, vly_kv* kv, const void* inputs_embeds, int B, int S, int logits_mode, void* logits_dev,
@@ -1551,9 +1548,7 @@ extern "C" int vly_llama_prefill(vly_ctx* c, vly_kv* kv, const void* inputs_embe
   TRY(ensure(c->w_pstats, (size_t)M * nt * sizeof(float2)));
   bf16 *x = (bf16*)c->w_x.p, *qb = (bf16*)c->w_q.p, *attn = (bf16*)c->w_attn.p, *hb = (bf16*)c->w_hb.p;
   float2* stats = (float2*)c->w_pstats.p;
-  copy_rows_stats_kernel<<<M, 128, 0, st>>>((const bf16*)inputs_embeds, x, stats, nt, H);
-  c->launches++;
-  CKL();
+  TRY(launch(c, copy_rows_stats_kernel, {dim3(M), dim3(128), 0, st}, (const bf16*)inputs_embeds, x, stats, nt, H));
   for (int l = 0; l < g.num_hidden_layers; ++l) {
     const LlamaLayerW& w = c->layers[l];
     {
@@ -1606,10 +1601,7 @@ extern "C" int vly_llama_prefill(vly_ctx* c, vly_kv* kv, const void* inputs_embe
   if (logits_mode == 1) CK(cudaMemcpyAsync(logits_dev, kv->logits, (size_t)B * V * 4, cudaMemcpyDeviceToDevice, st));
   if (next_tokens_dev) CK(cudaMemcpyAsync(next_tokens_dev, kv->cur_tokens, (size_t)B * 8, cudaMemcpyDeviceToDevice, st));
   kv->host_len = past + S;
-  set_int_kernel<<<1, 1, 0, st>>>(kv->d_len, kv->host_len);
-  c->launches++;
-  CKL();
-  return VLY_OK;
+  return launch(c, set_int_kernel, {dim3(1), dim3(1), 0, st}, kv->d_len, kv->host_len);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1627,23 +1619,11 @@ extern "C" int vly_kv_debug_counters(vly_kv* kv, long long* host_out, int n) {
 
 // the launch was planned by vly_kv_create (plan_decode_mega); filtered: sample_filter_kernel selects after the step
 static int launch_decode_mega(vly_ctx* c, vly_kv* kv, bool filtered, cudaStream_t st) {
-  const int bmax = kv->B <= 1 ? 1 : (kv->B <= 2 ? 2 : 4);
   StepParams p = kv->mega;
   p.select = filtered ? 0 : 1;
-  void* args[] = {&p};
-  cudaError_t e;
-#define VLY_MEGA_CASE(BM)                                                                                                          \
-  {                                                                                                                                \
-    TRY(ensure_smem_attr(c->cfg.device, decode_step_kernel<BM>, kv->mega_smem));                                                   \
-    e = cudaLaunchCooperativeKernel((void*)decode_step_kernel<BM>, dim3(c->num_sms), dim3(MegaCfg::THREADS), args, kv->mega_smem, st); \
-  }
-  if (bmax == 1) VLY_MEGA_CASE(1)
-  else if (bmax == 2) VLY_MEGA_CASE(2)
-  else VLY_MEGA_CASE(4)
-#undef VLY_MEGA_CASE
-  c->launches++;
-  CK(e);
-  return VLY_OK;
+  LaunchCfg l = {dim3(c->num_sms), dim3(MegaCfg::THREADS), kv->mega_smem, st};
+  l.cooperative = true;
+  return with_bmax(kv->B, [&](auto bm) { return launch(c, decode_step_kernel<decltype(bm)::value>, l, p); });
 }
 
 // token selection over [B, V] logits (sampling.cuh), one CTA per row; the scores of a filtered row are staged in shared memory
@@ -1651,12 +1631,8 @@ static int launch_sample_filter(vly_ctx* c, const float* logits, int B, int V, S
                                 long long* next_tokens, long long* out_tokens, int out_stride, bool filter, bool per_op,
                                 uint8_t* keep_out, cudaStream_t st) {
   const size_t smem = filter && (size_t)V * 4 <= (size_t)kFilterStageMaxBytes ? (size_t)V * 4 : 0;
-  TRY(ensure_smem_attr(c->cfg.device, sample_filter_kernel, smem));
-  sample_filter_kernel<<<B, kFilterThreads, smem, st>>>(logits, V, s, seq_len, step, next_tokens, out_tokens, out_stride, filter ? 1 : 0,
-                                                        per_op ? 1 : 0, keep_out);
-  c->launches++;
-  CKL();
-  return VLY_OK;
+  return launch(c, sample_filter_kernel, {dim3(B), dim3(kFilterThreads), smem, st}, logits, V, s, seq_len, step, next_tokens, out_tokens,
+                out_stride, filter ? 1 : 0, per_op ? 1 : 0, keep_out);
 }
 
 // filtered: the step ends with sample_filter_kernel's filtered selection (set_sampling)
@@ -1709,11 +1685,8 @@ static int set_sampling(vly_ctx* c, vly_kv* kv, const vly_sampling* sp, bool res
     // the filters apply only when sampling (HF ignores its warpers when it does not sample)
     kv->filtered = on && (sp->top_k > 0 || (sp->top_p > 0.f && sp->top_p < 1.f));
   }
-  set_sample_state_kernel<<<1, 64, 0, st>>>(kv->d_sample, r, reset_done ? 1 : 0);
   kv->sample_dirty = sp != nullptr;
-  c->launches++;
-  CKL();
-  return VLY_OK;
+  return launch(c, set_sample_state_kernel, {dim3(1), dim3(64), 0, st}, kv->d_sample, r, reset_done ? 1 : 0);
 }
 
 constexpr int kGraphSteps = 8;
@@ -1835,11 +1808,9 @@ extern "C" int vly_cross_entropy(vly_ctx* c, const float* logits, const int64_t*
   TRY(ensure(c->w_score, (size_t)rows * 8));
   float* nll = (float*)c->w_score.p;
   int* cnt = (int*)(nll + rows);
-  ce_rows_kernel<<<rows, 256, 0, st>>>(logits, (const long long*)labels, S, c->cfg.vocab_size, ignore_index, nll, cnt);
-  ce_mean_kernel<<<1, 1024, 0, st>>>(nll, cnt, rows, loss_out);
-  c->launches += 2;
-  CKL();
-  return VLY_OK;
+  TRY(launch(c, ce_rows_kernel, {dim3(rows), dim3(256), 0, st}, logits, (const long long*)labels, S, c->cfg.vocab_size, ignore_index, nll,
+             cnt));
+  return launch(c, ce_mean_kernel, {dim3(1), dim3(1024), 0, st}, nll, cnt, rows, loss_out);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1880,14 +1851,10 @@ extern "C" int vly_preprocess_frames(vly_ctx* c, const uint8_t* frames, int T, i
   }
   TRY(ensure(c->w_strip, (size_t)T * p.rows * 224 * 3));
   p.frames = frames; p.T = T; p.strip = (uint8_t*)c->w_strip.p; p.out = out; p.out_dtype = out_dtype;
-  preprocess_horizontal_kernel<<<dim3(p.rows, T), 224, 0, st>>>(p);
-  CKL();
-  if (out_dtype == VLY_F32) preprocess_vertical_kernel<float><<<dim3(224, T), 224, 0, st>>>(p);
-  else if (out_dtype == VLY_F16) preprocess_vertical_kernel<__half><<<dim3(224, T), 224, 0, st>>>(p);
-  else preprocess_vertical_kernel<__nv_bfloat16><<<dim3(224, T), 224, 0, st>>>(p);
-  CKL();
-  c->launches += 2;
-  return VLY_OK;
+  TRY(launch(c, preprocess_horizontal_kernel, {dim3(p.rows, T), dim3(224), 0, st}, p));
+  return with_dtype(out_dtype, [&](auto t) {
+    return launch(c, preprocess_vertical_kernel<typename decltype(t)::type>, {dim3(224, T), dim3(224), 0, st}, p);
+  });
 }
 
 // ------------------------------------------------------------------------------------------------
