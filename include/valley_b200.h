@@ -240,6 +240,24 @@ int vly_test_vit_attention(vly_ctx* ctx, const void* qkv_dev, int n_frames, void
  * computed by the same device routine the decode loop selects with.  temperature > 0; top_k / top_p as in vly_sampling. */
 int vly_test_sample_filter(vly_ctx* ctx, const float* logits_dev, int B, int V, float temperature, int top_k, float top_p,
                            uint8_t* keep_out_dev, void* stream);
+/* one weight-streaming GEMV of the per-op decode step, through the launcher the step uses: y[b,n] = sum_k x[b,k] W[n,k] with
+ * W [N,K] bf16, x [B,K] bf16 of row stride ldx (0 = K), B <= 4, K and ldx multiples of 8, W and x 16-byte aligned.  rstd[b] = 1/sqrt(mean_k x[b,k]^2 + eps)
+ * (the RMSNorm whose gamma is folded into W).  mode:
+ *   0 QKV + RoPE: rows in pair-interleaved RoPE order, N = 3 * nH * 128; rstd * y rotated by the RoPE table of the context at
+ *     position pos (0 <= pos < Smax): q -> out_dev [B, N/3]; k / v -> row pos of kcache_dev / vcache_dev [B, nH, Smax, 128]
+ *   1 residual: out_dev [B,N] = bf16(y + res_dev) (in place allowed)
+ *   2 SwiGLU: rows (2j, 2j+1) = (gate j, up j): out_dev [B,N/2] = silu(bf16(rstd*gate)) * bf16(rstd*up)
+ *   3 logits: logits_dev [B,N] fp32 (or NULL) = rstd * y; next_tokens_dev [B] int64 = arg-max (lowest index on ties)
+ * Arguments a mode does not use may be NULL / 0. */
+int vly_test_gemv(vly_ctx* ctx, int mode, const void* w_dev, const void* x_dev, int N, int K, int B, int64_t ldx, float eps,
+                  const void* res_dev, void* out_dev, void* kcache_dev, void* vcache_dev, int Smax, int pos, float* logits_dev,
+                  int64_t* next_tokens_dev, void* stream);
+/* the per-op decode step's attention, through the launcher the step uses: q_dev [B, nH*128] bf16 (RoPE pair-interleaved like the
+ * cache's keys), kcache_dev / vcache_dev [B, nH, Smax, 128] bf16 (Smax a multiple of 128), keys [0, len) with the newest at
+ * len - 1, key_mask_dev [B, len] uint8 (0 = key never attended) or NULL -> out_dev [B, nH*128] bf16 = softmax(q k^T / sqrt(128)) v
+ * over the attended keys.  B <= 4, nH <= 64. */
+int vly_test_decode_attention(vly_ctx* ctx, const void* q_dev, const void* kcache_dev, const void* vcache_dev, int B, int nH,
+                              int Smax, int len, const uint8_t* key_mask_dev, void* out_dev, void* stream);
 
 #ifdef __cplusplus
 }

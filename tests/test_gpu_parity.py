@@ -675,19 +675,30 @@ def test_cache_capacity_is_enforced():
         m(input_ids=ids.cuda(), past_key_values=cache)            # 2 x 327 > 384
 
 
-@pytest.mark.parametrize("spec_name,B", [("shape-13b-1l", 1), ("shape-13b-1l", 4), ("shape-7b-1l", 3)])
+@pytest.mark.parametrize("spec_name,B", [("shape-13b-1l", 1), ("shape-13b-1l", 4), ("shape-7b-1l", 3), ("shape-13b-1l", 5),
+                                         ("shape-13b-1l", 7), ("shape-13b-1l", 9), ("shape-7b-1l", 6)])
 def test_production_shapes_one_layer(spec_name, B):
     """One decoder layer at the real 7B / 13B widths (H 4096/5120, I 11008/13824, 32/40 heads, V 32008): prefill logits and
     6 teacher-forced decode steps vs the oracle -- covers the K-tail slices of the CUDA-core (B = 1) and tensor-core (B > 1)
-    decode consumers and the 128- / 256-wide GEMM tilings."""
+    decode consumers and the 128- / 256-wide GEMM tilings.  B > 4 runs the per-op kernels in groups of at most 4 rows:
+    4 + 1, 4 + 3, 4 + 4 + 1 and 4 + 2.  The oracle runs in fp32 on the GPU with TF32 off (the same plain-torch code as on
+    the CPU; a 9-row batch at 13B widths would take minutes there)."""
     spec = syn.SPECS[spec_name]
     sd = Hh.bf16_weights(spec, 2)
     m = Hh.build_model(spec, sd)
     cfg, tok = Hh.oracle_cfg(spec), Hh.oracle_tok(spec)
     T, n = 2, 6
     ids, px = syn.make_prompt_ids(spec, B, T, 0, len_a=12, len_b=7), syn.make_pixels(B, T, 0)
-    with torch.no_grad():
-        r_tok, r_log = O.greedy_generate(sd, cfg, tok, ids, px, n, return_logits=True)
+    tf32 = (torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32)
+    torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
+    try:
+        with torch.no_grad():
+            sd_dev = {k: v.cuda() for k, v in sd.items()}
+            r_tok, r_log = O.greedy_generate(sd_dev, cfg, tok, ids.cuda(), px.cuda(), n, return_logits=True)
+            r_tok, r_log = r_tok.cpu(), r_log.cpu()
+            del sd_dev
+    finally:
+        torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = tf32
     m.logits_all_positions = False
     out = m(input_ids=ids.cuda(), images=px.cuda())
     cache, logs = out.past_key_values, [out.logits[:, -1].cpu()]

@@ -90,6 +90,8 @@ SIGNATURES = {
     "vly_test_gemm": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp]),
     "vly_test_vit_attention": (_i, [_vp, _vp, _i, _vp, _vp]),
     "vly_test_sample_filter": (_i, [_vp, _vp, _i, _i, C.c_float, _i, C.c_float, _vp, _vp]),
+    "vly_test_gemv": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i64, C.c_float, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "vly_test_decode_attention": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
 }
 
 _lib = None

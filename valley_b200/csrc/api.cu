@@ -172,6 +172,8 @@ struct vly_ctx {
   Mem w_strip, w_tables;
   int pre_H = 0, pre_W = 0;
   PreprocParams pre = {};
+  // per-kernel test hooks: device scalars, work counters and partials of vly_test_gemv / vly_test_decode_attention
+  Mem w_tgemv, w_tattn;
 
   // (runs before the members above are freed)
   ~vly_ctx() {
@@ -1443,6 +1445,13 @@ static int launch_gemv_ring(vly_ctx* c, GemvParams p, bool pdl, cudaStream_t st)
   return with_bmax(p.B, [&](auto bm) { return launch(c, gemv_ring_kernel<decltype(bm)::value, MODE>, l, p, n_stages); });
 }
 
+// decode attention over the newest key *p.seq_len and the keys before it: one CTA per (row, head, 64-key split of Smax)
+static int launch_decode_attention(vly_ctx* c, DecAttnParams p, bool pdl, cudaStream_t st) {
+  p.nsplit = p.Smax / kDecSplitKeys;
+  p.scale_log2e = 0.08838834764831845f * 1.4426950408889634f;
+  return launch(c, decode_attention_v2_kernel, {dim3(p.B * p.nH, p.nsplit), dim3(128), 0, st, pdl, true}, p);
+}
+
 // Enqueue one decode step for batch rows [b0, b0+nb) of kv (nb <= 4).  Reads kv->cur_tokens, writes kv->cur_tokens.
 static int enqueue_decode_step(vly_ctx* c, vly_kv* kv, int b0, int nb, bool bump, cudaStream_t st) {
   const vly_config& g = c->cfg;
@@ -1462,15 +1471,13 @@ static int enqueue_decode_step(vly_ctx* c, vly_kv* kv, int b0, int nb, bool bump
     {
       DecAttnParams p = {};
       p.B = nb; p.nH = nH; p.H = H; p.Smax = kv->Smax; p.seq_len = kv->d_len;
-      p.nsplit = kv->Smax / kDecSplitKeys;
       p.q = q; p.kcache = kc; p.vcache = vc;
       p.part_o = kv->part_o + (size_t)b0 * nH * kv->nsplit * 128;
       p.part_ml = kv->part_ml + (size_t)b0 * nH * kv->nsplit;
       p.counters = kv->counters + (size_t)b0 * nH;
       p.out = attn;
-      p.scale_log2e = 0.08838834764831845f * 1.4426950408889634f;
       p.key_bits = kv->key_bits + (size_t)b0 * kv->mask_words(); p.mask_words = kv->mask_words();
-      TRY(launch(c, decode_attention_v2_kernel, {dim3(nb * nH, p.nsplit), dim3(128), 0, st, true, true}, p));
+      TRY(launch_decode_attention(c, p, true, st));
     }
     {
       GemvParams p = {};
@@ -1896,4 +1903,89 @@ extern "C" int vly_test_sample_filter(vly_ctx* c, const float* logits, int B, in
   TRY(ensure(c->w_score, sizeof(SampleState)));
   CK(cudaMemcpyAsync(c->w_score.p, &s, sizeof(s), cudaMemcpyHostToDevice, st));
   return launch_sample_filter(c, logits, B, V, (SampleState*)c->w_score.p, nullptr, nullptr, nullptr, nullptr, 0, true, false, keep_out, st);
+}
+
+// Grow-only scratch whose first `counter_bytes` are work counters: zeroed whenever the buffer is (re)allocated; the kernels
+// reset them to zero themselves at the end of every launch.
+static int ensure_counters(Mem& b, size_t bytes, size_t counter_bytes, cudaStream_t st) {
+  if (b.bytes >= bytes) return VLY_OK;
+  TRY(b.alloc(bytes));
+  CK(cudaMemsetAsync(b.p, 0, counter_bytes, st));
+  return VLY_OK;
+}
+
+extern "C" int vly_test_gemv(vly_ctx* c, int mode, const void* w, const void* x, int N, int K, int B, int64_t ldx, float eps,
+                             const void* res, void* out, void* kcache, void* vcache, int Smax, int pos, float* logits,
+                             int64_t* next_tokens, void* stream) {
+  if (!c || !w || !x || (((uintptr_t)w | (uintptr_t)x) & 15) || N <= 0 || K <= 0 || (K % 8) || B <= 0 || B > 4 || ldx < 0 ||
+      (ldx % 8) || (ldx > 0 && ldx < K))
+    return fail(VLY_ERR_INVALID, "vly_test_gemv: bad argument (N %d, K %d, B %d, ldx %lld)", N, K, B, (long long)ldx);
+  std::lock_guard<std::mutex> lk(c->mu);
+  CK(cudaSetDevice(c->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  GemvParams p = {};
+  p.N = N; p.K = K; p.B = B; p.W = (const bf16*)w; p.x = (const bf16*)x; p.ldx = ldx; p.eps = eps;
+  if (mode == GEMV_RESIDUAL) {
+    if (!res || !out) return fail(VLY_ERR_INVALID, "vly_test_gemv: the residual mode needs res and out");
+    p.res = (const bf16*)res; p.out = (bf16*)out;
+    return launch_gemv_ring<GEMV_RESIDUAL>(c, p, false, st);
+  }
+  if (mode == GEMV_SWIGLU) {
+    if (!out || (N % 2)) return fail(VLY_ERR_INVALID, "vly_test_gemv: the SwiGLU mode needs out and an even N");
+    p.out = (bf16*)out;
+    return launch_gemv_ring<GEMV_SWIGLU>(c, p, false, st);
+  }
+  // [0] position of the new token (QKV), [1] arg-max counter, [2] step, [3] length; then part_val, part_idx [B, grid]
+  const size_t part = (size_t)4 * c->num_sms * 4;
+  TRY(ensure_counters(c->w_tgemv, 16 + 2 * part, 16, st));
+  int* scal = (int*)c->w_tgemv.p;
+  if (mode == GEMV_QKV_ROPE) {
+    if (!out || !kcache || !vcache || (N % 384) || Smax <= 0 || pos < 0 || pos >= Smax || !c->rope ||
+        pos >= c->cfg.max_position_embeddings)
+      return fail(VLY_ERR_INVALID, "vly_test_gemv: the QKV mode needs out, K/V caches, N %% 384 == 0, 0 <= pos < Smax and a RoPE table");
+    CK(cudaMemcpyAsync(scal, &pos, sizeof(int), cudaMemcpyHostToDevice, st));
+    p.out = (bf16*)out; p.rope = c->rope; p.seq_len = scal; p.H = N / 3; p.nH = N / 384; p.Smax = Smax;
+    p.kcache = (bf16*)kcache; p.vcache = (bf16*)vcache;
+    return launch_gemv_ring<GEMV_QKV_ROPE>(c, p, false, st);
+  }
+  if (mode == GEMV_LOGITS) {
+    if (!next_tokens) return fail(VLY_ERR_INVALID, "vly_test_gemv: the logits mode needs next_tokens");
+    p.logits = logits;
+    p.counter = (unsigned int*)scal + 1;
+    p.step = scal + 2; p.seq_len_rw = scal + 3; p.bump = 0;
+    p.part_val = (float*)((uint8_t*)c->w_tgemv.p + 16);
+    p.part_idx = (int*)((uint8_t*)c->w_tgemv.p + 16 + part);
+    p.next_tokens = (long long*)next_tokens;
+    return launch_gemv_ring<GEMV_LOGITS>(c, p, false, st);
+  }
+  return fail(VLY_ERR_INVALID, "vly_test_gemv: unknown mode %d", mode);
+}
+
+extern "C" int vly_test_decode_attention(vly_ctx* c, const void* q, const void* kcache, const void* vcache, int B, int nH, int Smax,
+                                         int len, const uint8_t* key_mask, void* out, void* stream) {
+  constexpr int kMaxHeads = 4 * 64;           // counters for up to 4 rows x 64 heads: one per-op step group of the widest LLaMA
+  if (!c || !q || !kcache || !vcache || !out || B <= 0 || B > 4 || nH <= 0 || nH > 64 || Smax <= 0 || (Smax % 128) || len <= 0 ||
+      len > Smax)
+    return fail(VLY_ERR_INVALID, "vly_test_decode_attention: bad argument (B %d, heads %d, Smax %d, len %d)", B, nH, Smax, len);
+  std::lock_guard<std::mutex> lk(c->mu);
+  CK(cudaSetDevice(c->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int nsplit = Smax / kDecSplitKeys, words = Smax / 32, bh = B * nH;
+  // counters [kMaxHeads], seq_len, then key bits [B, words], part_ml [B*nH, nsplit], part_o [B*nH, nsplit, 128]
+  const size_t cnt = kMaxHeads * 4, off_bits = cnt + 16, bits = (size_t)B * words * 4;
+  const size_t off_ml = off_bits + ((bits + 15) & ~size_t(15)), off_o = off_ml + (size_t)bh * nsplit * sizeof(float2);
+  TRY(ensure_counters(c->w_tattn, off_o + (size_t)bh * nsplit * 128 * 4, cnt, st));
+  uint8_t* ws = (uint8_t*)c->w_tattn.p;
+  const int old_len = len - 1;
+  CK(cudaMemcpyAsync(ws + cnt, &old_len, sizeof(int), cudaMemcpyHostToDevice, st));
+  uint32_t* key_bits = (uint32_t*)(ws + off_bits);
+  if (key_mask) TRY(launch(c, pack_key_mask_kernel, {dim3(cdiv(words, 128), B), dim3(128), 0, st}, key_mask, len, words, key_bits));
+  else CK(cudaMemsetAsync(key_bits, 0xff, bits, st));
+  DecAttnParams p = {};
+  p.B = B; p.nH = nH; p.H = nH * 128; p.Smax = Smax; p.seq_len = (const int*)(ws + cnt);
+  p.q = (const bf16*)q; p.kcache = (const bf16*)kcache; p.vcache = (const bf16*)vcache;
+  p.part_o = (float*)(ws + off_o); p.part_ml = (float2*)(ws + off_ml); p.counters = (unsigned int*)ws;
+  p.out = (bf16*)out;
+  p.key_bits = key_bits; p.mask_words = words;
+  return launch_decode_attention(c, p, false, st);
 }
