@@ -1,6 +1,6 @@
 /* valley_b200.h -- C ABI of libvalley_b200.so: the H100-native (sm_90a) implementation of Valley's
  * multimodal forward hot path (CLIP ViT-L/14 encode -> temporal pool + mm_projector -> LLaMA decoder
- * with KV cache -> greedy token).
+ * with KV cache -> greedy, sampled or beam-searched tokens).
  *
  * The reference (RupertLuo/Valley) has NO FFI / plugin interface: the boundary it offers is the Python
  * nn.Module surface of valley/model/valley_model.py, whose arithmetic is delegated to HuggingFace
@@ -215,6 +215,34 @@ int vly_sample_logits(vly_ctx* ctx, vly_kv* kv, const float* logits_dev, const v
  * [0, steps_done) of out_tokens_dev are valid. */
 int vly_generate(vly_ctx* ctx, vly_kv* kv, const int64_t* first_tokens_dev, int n_steps, int64_t* out_tokens_dev,
                  const vly_sampling* sampling, int* steps_done_dev, void* stream);
+
+/* ---- beam search (HF generate with num_beams > 1, do_sample=False: transformers' GenerationMixin._beam_search) ----
+ * The cache holds B = items * num_beams rows, each item's beams prefilled with the same prompt (HF's
+ * _expand_inputs_for_generation).  Per step, on the device: log_softmax of every beam row + the running beam scores; the top
+ * 2 * num_beams of the num_beams * V candidates (ties: lowest flat index); a candidate hits the stopping criteria when its
+ * token is eos or at the last of n_steps steps; the next running beams are the best num_beams candidates that did not hit;
+ * the finished hypotheses keep the best num_beams by score / generated_len ** length_penalty under HF's early_stopping rules;
+ * the KV rows follow their parent beams (positions after the prompt only).  The search ends as HF's does, and the remaining
+ * graph replays then exit at once.  log_softmax uses a float64 log-sum-exp (within an ulp of the fp32 one). */
+typedef struct {
+  int32_t num_beams;             /* 1..8, divides the cache's rows                                              */
+  int32_t num_return_sequences;  /* 1..num_beams: the best finished hypotheses returned per item                 */
+  float length_penalty;          /* HF default 1.0                                                              */
+  int32_t early_stopping;        /* 0: False (HF default), 1: True, 2: "never"                                  */
+  int64_t eos_token_id;          /* -1: none                                                                    */
+  int64_t pad_token_id;          /* written beyond each sequence's end (HF's output_fill_value)                  */
+} vly_beam;
+
+/* Beam search after the prefill of the prompt_len-token prompt (the cache's length): the first step selects from
+ * first_logits_dev [B, V] fp32 (vly_llama_prefill logits_mode 1), each of the following n_steps - 1 steps is one CUDA-graph
+ * replay of decode step + beam_step_kernel + kv_beam_reorder_kernel.  Outputs, for item i and its r-th best hypothesis in
+ * row i * num_return_sequences + r: seq_out_dev [., n_steps] int64 (generated tokens, pad_token_id after the end),
+ * scores_out_dev [.] fp32 (HF's sequences_scores), gen_len_out_dev [.] int32 (generated length).  No host synchronisation. */
+int vly_beam_search(vly_ctx* ctx, vly_kv* kv, const vly_beam* params, const float* first_logits_dev, int prompt_len, int n_steps,
+                    int64_t* seq_out_dev, float* scores_out_dev, int* gen_len_out_dev, void* stream);
+/* HF's Cache.reorder_cache(beam_idx) for positions [from_pos, length): every layer's K and V row r takes row
+ * parent_rows_dev[r] (device int32 [B], any row of the cache), in place. */
+int vly_kv_beam_reorder(vly_ctx* ctx, vly_kv* kv, const int32_t* parent_rows_dev, int from_pos, void* stream);
 
 /* ---- introspection for bench / tests ---- */
 int vly_kernel_launch_count(vly_ctx* ctx, int64_t* out);   /* kernels launched by this ctx so far */

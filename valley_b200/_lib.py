@@ -41,6 +41,11 @@ class VlySampling(C.Structure):
         super().__init__(temperature, seed, eos_token_id, pad_token_id, stop_token_id, top_k, top_p)
 
 
+class VlyBeam(C.Structure):
+    _fields_ = [("num_beams", C.c_int32), ("num_return_sequences", C.c_int32), ("length_penalty", C.c_float),
+                ("early_stopping", C.c_int32), ("eos_token_id", C.c_int64), ("pad_token_id", C.c_int64)]
+
+
 VLY_OK, VLY_ERR_INVALID, VLY_ERR_CUDA, VLY_ERR_STATE = 0, -1, -2, -3
 VLY_ERR_IM_COUNT, VLY_ERR_IM_CUT, VLY_ERR_INDEX = -10, -11, -12
 VLY_F32, VLY_BF16, VLY_F16 = 0, 1, 2
@@ -82,6 +87,8 @@ SIGNATURES = {
     "vly_cross_entropy": (_i, [_vp, _vp, _vp, _i, _i, _i64, _vp, _vp]),
     "vly_sample_logits": (_i, [_vp, _vp, _vp, _p(VlySampling), _vp, _vp]),
     "vly_generate": (_i, [_vp, _vp, _vp, _i, _vp, _p(VlySampling), _vp, _vp]),
+    "vly_beam_search": (_i, [_vp, _vp, _p(VlyBeam), _vp, _i, _i, _vp, _vp, _vp, _vp]),
+    "vly_kv_beam_reorder": (_i, [_vp, _vp, _vp, _i, _vp]),
     "vly_kernel_launch_count": (_i, [_vp, _p(_i64)]),
     "vly_held_bytes": (_i, [_p(_i64), _p(_i64)]),
     "vly_num_sms": (_i, [_vp, _p(_i)]),

@@ -27,6 +27,7 @@
 #include "decode_mega.cuh"
 #include "preprocess.cuh"
 #include "pooling_kernels.cuh"
+#include "beam.cuh"
 
 using namespace vly;
 typedef __nv_bfloat16 bf16;
@@ -221,6 +222,15 @@ struct vly_kv {
   // kernel->kernel edges inside)]; each pair is captured on first use
   cudaGraphExec_t graph[2][2] = {};
   int graph_nodes[2] = {};            // kernel launches per step of each pair
+  // beam search (vly_beam_search), allocated on the cache's first beam request: the state, the running and finished token
+  // rows [2 parities][2][B][Smax] and the length-penalty divisors [Smax]; the step graphs (one step, kGraphSteps steps) are
+  // captured for beam_graph_nb beams per item
+  Owned<BeamState> d_beam;
+  Owned<long long> beam_tok;
+  Owned<float> beam_div;
+  Owned<int> beam_from;               // vly_kv_beam_reorder's first position
+  cudaGraphExec_t beam_graph[2] = {};
+  int beam_graph_nb = 0, beam_nodes = 0;
   size_t layer_stride() const { return (size_t)2 * B * ctx->cfg.num_attention_heads * Smax * 128; }
   bf16* k_layer(int l) const { return cache + (size_t)l * layer_stride(); }
   bf16* v_layer(int l) const { return k_layer(l) + layer_stride() / 2; }
@@ -230,6 +240,8 @@ struct vly_kv {
     for (auto& pair : graph)
       for (cudaGraphExec_t g : pair)
         if (g) cudaGraphExecDestroy(g);
+    for (cudaGraphExec_t g : beam_graph)
+      if (g) cudaGraphExecDestroy(g);
     if (len_event) cudaEventDestroy(len_event);
   }
 };
@@ -1697,14 +1709,16 @@ static int set_sampling(vly_ctx* c, vly_kv* kv, const vly_sampling* sp, bool res
 }
 
 constexpr int kGraphSteps = 8;
-static int capture_steps(vly_ctx* c, vly_kv* kv, int n, bool filtered, cudaGraphExec_t* out) {
+// n steps of enqueue_step(stream) as one graph; *nodes receives the kernel launches per step
+template <typename F>
+static int capture_steps(vly_ctx* c, int n, F&& enqueue_step, cudaGraphExec_t* out, int* nodes) {
   const int64_t before = c->launches;
   CK(cudaStreamBeginCapture(c->cap_stream, cudaStreamCaptureModeThreadLocal));
   int r = VLY_OK;
-  for (int i = 0; i < n && r == VLY_OK; ++i) r = enqueue_full_step(c, kv, filtered, c->cap_stream);
+  for (int i = 0; i < n && r == VLY_OK; ++i) r = enqueue_step(c->cap_stream);
   cudaGraph_t graph = nullptr;
   const cudaError_t e = cudaStreamEndCapture(c->cap_stream, &graph);
-  kv->graph_nodes[filtered] = (int)((c->launches - before) / n);
+  *nodes = (int)((c->launches - before) / n);
   c->launches = before;
   if (r != VLY_OK) {
     if (graph) cudaGraphDestroy(graph);
@@ -1719,8 +1733,9 @@ static int capture_steps(vly_ctx* c, vly_kv* kv, int n, bool filtered, cudaGraph
 static int build_graph(vly_ctx* c, vly_kv* kv, bool filtered) {
   cudaGraphExec_t* g = kv->graph[filtered];
   if (g[0]) return VLY_OK;
-  TRY(capture_steps(c, kv, 1, filtered, &g[0]));
-  TRY(capture_steps(c, kv, kGraphSteps, filtered, &g[1]));
+  auto step = [&](cudaStream_t st) { return enqueue_full_step(c, kv, filtered, st); };
+  TRY(capture_steps(c, 1, step, &g[0], &kv->graph_nodes[filtered]));
+  TRY(capture_steps(c, kGraphSteps, step, &g[1], &kv->graph_nodes[filtered]));
   return VLY_OK;
 }
 
@@ -1800,6 +1815,109 @@ extern "C" int vly_llama_decode(vly_ctx* c, vly_kv* kv, const int64_t* tokens, i
   if (logits_dev) CK(cudaMemcpyAsync(logits_dev, kv->logits, (size_t)kv->B * c->cfg.vocab_size * 4, cudaMemcpyDeviceToDevice, st));
   kv->host_len += 1;
   return VLY_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// beam search (beam.cuh)
+// ------------------------------------------------------------------------------------------------
+static int ensure_beam_buffers(vly_kv* kv) {
+  if (kv->d_beam) return VLY_OK;
+  TRY(kv->d_beam.alloc(sizeof(BeamState)));
+  TRY(kv->beam_tok.alloc((size_t)4 * kv->B * kv->Smax * sizeof(long long)));
+  TRY(kv->beam_div.alloc((size_t)kv->Smax * sizeof(float)));
+  TRY(kv->beam_from.alloc(sizeof(int)));
+  return VLY_OK;
+}
+
+// rows within groups of `group` take their parent's positions [*from_pos, *len) (kv_beam_reorder_kernel)
+static int launch_kv_beam_reorder(vly_ctx* c, vly_kv* kv, int group, const int* parent, const int* from_pos, const int* skip,
+                                  cudaStream_t st) {
+  const int nH = c->cfg.num_attention_heads, L = c->cfg.num_hidden_layers;
+  const size_t smem = (size_t)group * reorder_block_positions(group) * 256;
+  return launch(c, kv_beam_reorder_kernel, {dim3(L * 2 * (kv->B / group) * nH), dim3(kReorderThreads), smem, st}, kv->cache, kv->B,
+                nH, kv->Smax, group, parent, from_pos, (const int*)kv->d_len, skip);
+}
+
+static int launch_beam_step(vly_ctx* c, vly_kv* kv, int nb, const float* logits, cudaStream_t st) {
+  long long* fin = kv->beam_tok + (size_t)2 * kv->B * kv->Smax;
+  return launch(c, beam_step_kernel, {dim3(kv->B / nb), dim3(kBeamThreads), 0, st}, logits, c->cfg.vocab_size, kv->d_beam,
+                (long long*)kv->beam_tok, fin, kv->Smax, (const float*)kv->beam_div, (long long*)kv->cur_tokens, kv->d_sample);
+}
+
+// one decode step of a beam request: the step writes the logits (select = 0), beam_step_kernel selects, the cache follows the
+// parents
+static int enqueue_beam_step(vly_ctx* c, vly_kv* kv, int nb, cudaStream_t st) {
+  if (kv->B <= 4) {
+    TRY(launch_decode_mega(c, kv, true, st));
+  } else {
+    for (int b0 = 0; b0 < kv->B; b0 += 4) TRY(enqueue_decode_step(c, kv, b0, std::min(4, kv->B - b0), b0 + 4 >= kv->B, st));
+  }
+  TRY(launch_beam_step(c, kv, nb, kv->logits, st));
+  return launch_kv_beam_reorder(c, kv, nb, kv->d_beam->parent, &kv->d_beam->prompt_len, &kv->d_beam->done, st);
+}
+
+extern "C" int vly_beam_search(vly_ctx* c, vly_kv* kv, const vly_beam* bp, const float* first_logits, int prompt_len, int n_steps,
+                               int64_t* seq_out, float* scores_out, int* gen_len_out, void* stream) {
+  if (!c || !kv || !bp || !first_logits || !seq_out || !scores_out || !gen_len_out || n_steps <= 0 || kv->ctx != c)
+    return fail(VLY_ERR_INVALID, "vly_beam_search: bad argument");
+  const int nb = bp->num_beams, nrs = bp->num_return_sequences;
+  if (nb < 1 || nb > kMaxBeams || kv->B % nb != 0)
+    return fail(VLY_ERR_INVALID, "vly_beam_search: num_beams %d must be in [1, %d] and divide the cache's %d rows", nb, kMaxBeams, kv->B);
+  if (kv->B > kMaxSampleRows) return fail(VLY_ERR_INVALID, "vly_beam_search: at most %d rows per cache (%d)", kMaxSampleRows, kv->B);
+  if (nrs < 1 || nrs > nb) return fail(VLY_ERR_INVALID, "vly_beam_search: num_return_sequences %d must be in [1, num_beams %d]", nrs, nb);
+  if (bp->early_stopping < 0 || bp->early_stopping > 2) return fail(VLY_ERR_INVALID, "vly_beam_search: early_stopping %d", bp->early_stopping);
+  std::lock_guard<std::mutex> lk(c->mu);
+  TRY(sync_len(kv));
+  if (prompt_len != kv->host_len) return fail(VLY_ERR_STATE, "vly_beam_search: the cache holds %d tokens, not the %d-token prompt", kv->host_len, prompt_len);
+  if (kv->host_len + n_steps - 1 > kv->Smax) return fail(VLY_ERR_INVALID, "vly_beam_search: %d cached + %d steps exceed the cache capacity %d", kv->host_len, n_steps - 1, kv->Smax);
+  CK(cudaSetDevice(c->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  TRY(ensure_beam_buffers(kv));
+  if (kv->beam_graph_nb != nb) {
+    for (cudaGraphExec_t& g : kv->beam_graph) {
+      if (g) cudaGraphExecDestroy(g);
+      g = nullptr;
+    }
+    auto step = [&](cudaStream_t s) { return enqueue_beam_step(c, kv, nb, s); };
+    TRY(capture_steps(c, 1, step, &kv->beam_graph[0], &kv->beam_nodes));
+    TRY(capture_steps(c, kGraphSteps, step, &kv->beam_graph[1], &kv->beam_nodes));
+    kv->beam_graph_nb = nb;
+  }
+  // plain selection state: the decode steps write logits only, and exit once beam_step_kernel raises all_done
+  kv->filtered = false;
+  kv->sample_dirty = true;            // (all_done stays raised after the search: the next request resets the state)
+  TRY(launch(c, set_sample_state_kernel, {dim3(1), dim3(64), 0, st}, kv->d_sample, SampleState{}, 1));
+  TRY(launch(c, beam_init_kernel, {dim3(1), dim3(256), 0, st}, kv->d_beam, kv->B, nb, n_steps, prompt_len, (int)bp->early_stopping,
+             bp->length_penalty, (long long)(bp->eos_token_id < 0 ? -1 : bp->eos_token_id), (float*)kv->beam_div));
+  TRY(launch_beam_step(c, kv, nb, first_logits, st));
+  CK(cudaMemsetAsync(kv->d_step, 0, 4, st));
+  for (int i = 0; i < n_steps - 1;) {
+    if (n_steps - 1 - i >= kGraphSteps) { CK(cudaGraphLaunch(kv->beam_graph[1], st)); i += kGraphSteps; }
+    else { CK(cudaGraphLaunch(kv->beam_graph[0], st)); ++i; }
+  }
+  c->launches += (int64_t)(n_steps - 1) * kv->beam_nodes;
+  const long long* fin = kv->beam_tok + (size_t)2 * kv->B * kv->Smax;
+  TRY(launch(c, beam_output_kernel, {dim3(kv->B / nb * nrs), dim3(256), 0, st}, (const BeamState*)kv->d_beam, fin, kv->Smax, kv->B, nrs,
+             n_steps, (long long)bp->pad_token_id, (long long*)seq_out, scores_out, gen_len_out));
+  // the steps after the end of the search did not advance the cache: the device holds its length
+  kv->host_len += n_steps - 1;
+  CK(cudaMemcpyAsync(kv->h_len, kv->d_len, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaEventRecord(kv->len_event, st));
+  kv->len_dirty = true;
+  return VLY_OK;
+}
+
+extern "C" int vly_kv_beam_reorder(vly_ctx* c, vly_kv* kv, const int32_t* parent_rows, int from_pos, void* stream) {
+  if (!c || !kv || !parent_rows || kv->ctx != c || from_pos < 0) return fail(VLY_ERR_INVALID, "vly_kv_beam_reorder: bad argument");
+  if (kv->B > kMaxSampleRows) return fail(VLY_ERR_INVALID, "vly_kv_beam_reorder: at most %d rows per cache (%d)", kMaxSampleRows, kv->B);
+  TRY(sync_len(kv));
+  std::lock_guard<std::mutex> lk(c->mu);
+  if (from_pos >= kv->host_len) return VLY_OK;
+  CK(cudaSetDevice(c->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  TRY(ensure_beam_buffers(kv));
+  TRY(launch(c, set_int_kernel, {dim3(1), dim3(1), 0, st}, (int*)kv->beam_from, from_pos));
+  return launch_kv_beam_reorder(c, kv, kv->B, parent_rows, kv->beam_from, nullptr, st);
 }
 
 // ------------------------------------------------------------------------------------------------

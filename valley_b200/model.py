@@ -21,7 +21,8 @@ from typing import Iterable, List, Optional, Tuple, Union
 import torch
 
 from . import _lib
-from ._lib import VlySampling, VlyConfig, VlyTokens, check
+from . import beam as _beam
+from ._lib import VlyBeam, VlySampling, VlyConfig, VlyTokens, check
 
 # valley/util/config.py:1-13
 IGNORE_INDEX = -100
@@ -161,6 +162,14 @@ class ValleyKVCache:
 
     def reset(self):
         check(self._model._lib.vly_kv_reset(self._h, _stream()))
+
+    def reorder_cache(self, beam_idx: torch.Tensor, from_pos: int = 0):
+        """HF's ``Cache.reorder_cache(beam_idx)``: row r of every layer's keys and values becomes row ``beam_idx[r]``, in place
+        on the device.  Positions before ``from_pos`` are left alone (a beam search's prompt rows are identical)."""
+        idx = beam_idx.to(self._model.device, torch.int32).contiguous()
+        if idx.shape != (self.batch,):
+            raise ValueError(f"beam_idx shape {tuple(idx.shape)} != ({self.batch},)")
+        check(self._model._lib.vly_kv_beam_reorder(self._model._ctx, self._h, idx.data_ptr(), int(from_pos), _stream()))
 
     def set_attention_mask(self, attention_mask: Optional[torch.Tensor], total_len: int):
         """HF's 2-D ``attention_mask`` [B, total_len] over cache positions 0..total_len-1 (past + new): a 0 means
@@ -320,6 +329,11 @@ class KeywordsStoppingCriteria:
 
 
 _UNSET = object()
+
+
+def _repeat_rows(t: torch.Tensor, n: int) -> torch.Tensor:
+    """every row n times in a row (HF's _expand_inputs_for_generation), without a host synchronisation"""
+    return t[:, None].expand(t.shape[0], n, *t.shape[1:]).reshape(t.shape[0] * n, *t.shape[1:]).contiguous()
 
 
 def sampling_filters(top_k=None, top_p=None) -> Tuple[int, float]:
@@ -716,7 +730,8 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
 
     @torch.no_grad()
     def generate(self, input_ids=None, images=None, max_new_tokens: int = 1024, do_sample: bool = False,
-                 temperature: float = 1.0, stopping_criteria=None, eos_token_id=_UNSET, top_k=None, top_p=None, **kw):
+                 temperature: float = 1.0, stopping_criteria=None, eos_token_id=_UNSET, top_k=None, top_p=None,
+                 num_beams: int = 1, num_return_sequences: int = 1, length_penalty: float = 1.0, early_stopping=False, **kw):
         """Greedy (or temperature) generation == the loop of model_worker.py:371-397 / HF generate as called at
         valley_model.py:432.  Returns [B, S + n_new] like HF.  With no stopping criteria, decoding runs
         entirely on the device (CUDA-graph replay, no per-token host sync).  ``attention_mask`` [B, S] (left padding)
@@ -729,8 +744,18 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
         HF defaults that the reference's callers rely on are kept: ``eos_token_id`` / ``pad_token_id`` default to the config's
         (generation stops when every row has emitted eos; finished rows are padded), and when no ``attention_mask`` is given
         but the prompt contains ``pad_token_id`` (!= eos) the mask is inferred as ``input_ids != pad_token_id``
-        (HF:generation/utils.py _prepare_attention_mask_for_generation).  Pass ``eos_token_id=None`` to run the full length."""
+        (HF:generation/utils.py _prepare_attention_mask_for_generation).  Pass ``eos_token_id=None`` to run the full length.
+
+        ``num_beams > 1`` runs HF's beam search (``length_penalty``, ``early_stopping`` True / False / "never",
+        ``num_return_sequences`` best hypotheses per row, returned as [B * num_return_sequences, S + L]).  Without stopping
+        criteria (and up to 8 beams and 64 rows in all) the selection and the KV-cache reorder run inside the decode step's CUDA
+        graph, with one device-to-host read per request; otherwise a host-visible loop runs the same search
+        (valley_b200/beam.py).  The returned sequences' scores (HF's ``sequences_scores``) are left in
+        ``model.last_beam_scores``.  Beam sampling (``do_sample=True``) is not implemented."""
         B, S = input_ids.shape
+        if num_beams != 1:
+            return self._beam_generate(input_ids, images, max_new_tokens, do_sample, stopping_criteria, eos_token_id, num_beams,
+                                       num_return_sequences, length_penalty, early_stopping, **kw)
         greedy = (not do_sample) or temperature < 1e-4
         filters = {} if greedy else dict(zip(("top_k", "top_p"), sampling_filters(top_k, top_p)))
         room = self.config.max_position_embeddings - S
@@ -811,6 +836,79 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
             if i + 1 < n_new:
                 logits, nxt = self._decode(cache, nxt, not greedy)
         return seq
+
+    def _beam_generate(self, input_ids, images, max_new_tokens, do_sample, stopping_criteria, eos_token_id, num_beams,
+                       num_return_sequences, length_penalty, early_stopping, **kw):
+        """generate(num_beams > 1): the vision part is encoded once per row, then every row's embeddings and attention mask
+        are repeated num_beams times (HF's _expand_inputs_for_generation) and prefilled as B * num_beams cache rows."""
+        if not isinstance(num_beams, int) or num_beams < 1:
+            raise ValueError(f"`num_beams` has to be a strictly positive integer, but is {num_beams}")
+        if do_sample:
+            raise NotImplementedError("beam sampling (num_beams > 1 with do_sample=True) is not implemented")
+        if not isinstance(num_return_sequences, int) or not 1 <= num_return_sequences <= num_beams:
+            raise ValueError(f"`num_return_sequences` ({num_return_sequences}) has to be smaller or equal to `num_beams` ({num_beams}).")
+        if early_stopping not in (True, False, "never"):
+            raise ValueError(f"`early_stopping` must be a boolean or 'never', but is {early_stopping}.")
+        B, S = input_ids.shape
+        nb = num_beams
+        n_new = max(0, min(max_new_tokens, self.config.max_position_embeddings - S))
+        ids_dev = input_ids.to(self.device, torch.int64)
+        if n_new == 0:
+            return _repeat_rows(ids_dev, num_return_sequences)
+        if eos_token_id is _UNSET:
+            eos_token_id = getattr(self.config, "eos_token_id", None)
+        pad_token_id = kw.get("pad_token_id", getattr(self.config, "pad_token_id", None))
+        if pad_token_id is None and eos_token_id is not None:
+            pad_token_id = eos_token_id                       # HF generate: pad defaults to eos
+        attention_mask = kw.get("attention_mask")
+        if attention_mask is None and pad_token_id is not None and (eos_token_id is None or pad_token_id != eos_token_id):
+            is_pad = input_ids == pad_token_id
+            if bool(is_pad.any()):
+                attention_mask = (~is_pad).to(torch.int64)
+        fill = _beam.output_fill_value(pad_token_id, eos_token_id)
+        _, _, _, embeds, _ = self.prepare_inputs_labels_for_multimodal(input_ids, None, None, None, images)
+        embeds = _repeat_rows(embeds, nb)
+        ids_rep = _repeat_rows(ids_dev, nb)
+        if attention_mask is not None:
+            attention_mask = _repeat_rows(attention_mask, nb)
+        cache = self._borrow_cache(B * nb)
+        try:
+            cache.set_attention_mask(attention_mask, S)
+            logits, _ = self._prefill(cache, embeds, 1)
+            logits = logits[:, -1].contiguous()
+            if not stopping_criteria and nb <= 8 and B * nb <= 64:
+                nrs = num_return_sequences
+                es = {False: 0, True: 1, "never": 2}[early_stopping]
+                bp = VlyBeam(nb, nrs, float(length_penalty), es, -1 if eos_token_id is None else int(eos_token_id), fill)
+                seq = torch.empty(B * nrs, n_new, dtype=torch.int64, device=self.device)
+                scores = torch.empty(B * nrs, dtype=torch.float32, device=self.device)
+                lens = torch.empty(B * nrs, dtype=torch.int32, device=self.device)
+                check(self._lib.vly_beam_search(self._ctx, cache._h, C.byref(bp), logits.data_ptr(), S, n_new, seq.data_ptr(),
+                                                scores.data_ptr(), lens.data_ptr(), _stream()))
+                L = int(lens.max())                          # the request's one device-to-host read
+                self.last_beam_scores = scores
+                return torch.cat([_repeat_rows(ids_dev, nrs), seq[:, :L]], dim=1)
+            # host-visible loop: the same search in torch over the library's logits, with HF's stopping criteria on the
+            # candidates (a criterion returning a plain bool applies to every row, as in HF's StoppingCriteriaList)
+            bs = _beam.BeamSearch(ids_rep, nb, n_new, eos_token_id, fill, length_penalty, early_stopping)
+            stop = None
+            if stopping_criteria:
+                def stop(seqs):
+                    done = torch.zeros(seqs.shape[0], dtype=torch.bool, device=seqs.device)
+                    for sc in stopping_criteria:
+                        done = done | torch.as_tensor(sc(seqs, None), device=seqs.device)
+                    return done
+            while True:
+                parents, tokens = bs.step(logits, stop)
+                if bs.done:
+                    break
+                cache.reorder_cache(parents, from_pos=S)
+                step_logits, _ = self._decode(cache, tokens, True)
+                logits = step_logits[:, -1]
+            out, self.last_beam_scores = bs.result(num_return_sequences)
+            return out
+        finally:
+            self._return_cache(cache)
 
     # ---------------- prompt helpers (pure string logic; valley_model.py:381-422) ----------------
     def build_inputs(self, tokenizer, messages):
