@@ -14,8 +14,11 @@
  *     the library owns only its packed weights, workspace and KV caches (tied to vly_ctx / vly_kv).
  *   - calls are stream-ordered on the cudaStream_t passed in (void* stream; NULL = legacy default stream).
  *   - there is NO CPU fallback: without a CUDA device of compute capability 9.x vly_create fails.
- *   - hot calls do not allocate once the workspace has grown to the largest shapes seen, so the decode
- *     step is captured in a CUDA graph (vly_generate_greedy).
+ *   - hot calls do not allocate once the workspace has grown to the largest shapes seen, so decode steps run
+ *     as CUDA graph replays: a KV cache captures a 1-step and an 8-step graph per kind of step (token, filtered
+ *     token, beam search step) on the kind's first use, the beam graphs again for another beam count, and
+ *     vly_llama_decode, vly_generate(_greedy) and vly_beam_search replay them.  VLY_NO_GRAPH=1 (profiling)
+ *     launches the steps eagerly instead.
  *   - thread safety: a vly_ctx serialises its workspace-using calls with an internal mutex
  *     (model_worker.py:467-474 may call the model from up to 5 threads); distinct vly_kv are independent.
  */

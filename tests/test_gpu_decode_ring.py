@@ -1,8 +1,9 @@
 """GPU: the persistent decode kernel's settings (DecodeSettings in api.cu: VLY_MEGA_*, VLY_ATTN_IKEYS) are read when a KV
 cache is created and stay with that cache.  Those tested here change only scheduling -- the L2 eviction hint on the weight
-stream, the ring depth, the bytes of copies in flight -- never what is computed: logits and token ids must be equal bit for
-bit to those of the reference configuration.  Each configuration runs in a subprocess of its own on the same seeded weights
-and prompt; one in-process test checks that a cache keeps its settings when the environment changes."""
+stream, the ring depth, the bytes of copies in flight, and (VLY_NO_GRAPH) eager launches instead of graph replays -- never
+what is computed: logits, greedy, sampled and beam token ids and beam scores must be equal bit for bit to those of the
+reference configuration.  Each configuration runs in a subprocess of its own on the same seeded weights and prompt; one
+in-process test checks that a cache keeps its settings when the environment changes."""
 import os
 import subprocess
 import sys
@@ -39,8 +40,16 @@ with torch.no_grad():
     gen = torch.empty(B, n, dtype=torch.int64, device="cuda")
     check(m._lib.vly_generate_greedy(m._ctx, cache._h, nxt.data_ptr(), n, gen.data_ptr(), 0))
     torch.cuda.synchronize()
+    seq_len = cache.get_seq_length()
+    # seeded sampling through a top-k filter, then a 2-beam search on the device: 11 steps each after the first token,
+    # one 8-step graph and three 1-step graphs
+    torch.manual_seed(11)
+    sampled = m.generate(input_ids=ids.cuda(), max_new_tokens=12, do_sample=True, temperature=0.8, top_k=20, eos_token_id=None)
+    beam = m.generate(input_ids=ids[:max(B // 2, 1)].cuda(), max_new_tokens=12, num_beams=2, eos_token_id=None)
+    beam_scores = m.last_beam_scores
 np.savez(out_path, logits=torch.stack(logs, 1).numpy(), tokens=torch.cat(tok, 1).numpy(), gen=gen.cpu().numpy(),
-         seq_len=np.array([cache.get_seq_length()]))
+         seq_len=np.array([seq_len]), sampled=sampled.cpu().numpy(), beam=beam.cpu().numpy(),
+         beam_scores=beam_scores.float().cpu().numpy())
 """
 
 # the plain ring (no hint) first: the reference of the others
@@ -49,6 +58,7 @@ CONFIGS = {
     "defaults": {},
     "2 stages": {"VLY_MEGA_STAGES": "2"},
     "64 KB in flight": {"VLY_MEGA_INFLIGHT_KB": "64"},
+    "eager": {"VLY_NO_GRAPH": "1"},
 }
 SETTINGS = ("VLY_MEGA_STAGE_KB", "VLY_MEGA_ROWS", "VLY_MEGA_INFLIGHT_KB", "VLY_MEGA_STAGES", "VLY_MEGA_INFLIGHT", "VLY_ATTN_IKEYS",
             "VLY_MEGA_L2_HINT", "VLY_MEGA_DBG")
@@ -56,7 +66,7 @@ SETTINGS = ("VLY_MEGA_STAGE_KB", "VLY_MEGA_ROWS", "VLY_MEGA_INFLIGHT_KB", "VLY_M
 
 def _run(tmp_path, spec_name, B, S, name, env_over):
     env = dict(os.environ)
-    for k in SETTINGS + ("VLY_LIB_PATH",):
+    for k in SETTINGS + ("VLY_LIB_PATH", "VLY_NO_GRAPH"):
         env.pop(k, None)
     env.update(env_over)
     out = str(tmp_path / f"{spec_name}_{B}_{name.replace(' ', '_').replace('/', '')}.npz")
@@ -80,6 +90,10 @@ def test_decode_ring_options_are_bit_identical(tmp_path, spec_name, B, S):
         assert np.array_equal(got["logits"].view(np.uint32), ref["logits"].view(np.uint32)), f"{spec_name} B={B}: logits differ with {name}"
         assert np.array_equal(got["tokens"], ref["tokens"]), f"{spec_name} B={B}: token ids differ with {name}"
         assert np.array_equal(got["gen"], ref["gen"]), f"{spec_name} B={B}: generated ids differ with {name}"
+        assert np.array_equal(got["sampled"], ref["sampled"]), f"{spec_name} B={B}: sampled ids differ with {name}"
+        assert np.array_equal(got["beam"], ref["beam"]), f"{spec_name} B={B}: beam ids differ with {name}"
+        assert np.array_equal(got["beam_scores"].view(np.uint32), ref["beam_scores"].view(np.uint32)), \
+            f"{spec_name} B={B}: beam scores differ with {name}"
 
 
 def test_decode_settings_are_fixed_per_cache(monkeypatch):

@@ -1,5 +1,5 @@
 // libvalley_b200.so -- host side of the C ABI declared in include/valley_b200.h.
-// Owns: packed weights, workspace, KV caches, CUDA-graph of the decode step.  No torch, no CPU fallback.
+// Owns: packed weights, workspace, KV caches, CUDA graphs of the decode steps.  No torch, no CPU fallback.
 #include <cuda_runtime.h>
 #include <cuda.h>
 
@@ -184,6 +184,24 @@ struct vly_ctx {
   }
 };
 
+// What a decode step ends with: the token selected by the persistent kernel or the per-op path's selection kernel, a filtered
+// token (sample_filter_kernel after the step), or a beam search step (beam_step_kernel + kv_beam_reorder_kernel)
+enum StepKind { STEP_TOKEN, STEP_FILTERED, STEP_BEAM, kStepKinds };
+
+// The decode steps of one kind as CUDA graphs: one step, and kGraphSteps steps in one graph (fewer graph launches,
+// kernel->kernel edges inside).  Captured on first use, and again for another beam count; the only owner of graph execs.
+struct StepGraphs {
+  cudaGraphExec_t one = nullptr, many = nullptr;
+  int nodes = 0;                      // kernel launches per step
+  int nb = 0;                         // beams per item the beam steps were captured for
+  void reset() {
+    if (one) cudaGraphExecDestroy(one);
+    if (many) cudaGraphExecDestroy(many);
+    one = many = nullptr;
+  }
+  ~StepGraphs() { reset(); }
+};
+
 struct vly_kv;
 static int sync_len(vly_kv* kv);
 struct vly_kv {
@@ -218,30 +236,18 @@ struct vly_kv {
   Owned<uint32_t> key_bits;           // [B, Smax/32] attention_mask bits (1 = attend); all ones unless vly_kv_set_key_mask
   bool masked = false;
   int mask_words() const { return Smax / 32; }
-  // the decode step as CUDA graphs, [filtered][0: one step, 1: kGraphSteps steps in one graph (fewer graph launches,
-  // kernel->kernel edges inside)]; each pair is captured on first use
-  cudaGraphExec_t graph[2][2] = {};
-  int graph_nodes[2] = {};            // kernel launches per step of each pair
   // beam search (vly_beam_search), allocated on the cache's first beam request: the state, the running and finished token
-  // rows [2 parities][2][B][Smax] and the length-penalty divisors [Smax]; the step graphs (one step, kGraphSteps steps) are
-  // captured for beam_graph_nb beams per item
+  // rows [2 parities][2][B][Smax] and the length-penalty divisors [Smax]
   Owned<BeamState> d_beam;
   Owned<long long> beam_tok;
   Owned<float> beam_div;
   Owned<int> beam_from;               // vly_kv_beam_reorder's first position
-  cudaGraphExec_t beam_graph[2] = {};
-  int beam_graph_nb = 0, beam_nodes = 0;
+  StepGraphs graphs[kStepKinds];      // (declared after the buffers they refer to: destroyed before them)
   size_t layer_stride() const { return (size_t)2 * B * ctx->cfg.num_attention_heads * Smax * 128; }
   bf16* k_layer(int l) const { return cache + (size_t)l * layer_stride(); }
   bf16* v_layer(int l) const { return k_layer(l) + layer_stride() / 2; }
 
-  // (runs before the buffers the graphs and the event refer to are freed)
   ~vly_kv() {
-    for (auto& pair : graph)
-      for (cudaGraphExec_t g : pair)
-        if (g) cudaGraphExecDestroy(g);
-    for (cudaGraphExec_t g : beam_graph)
-      if (g) cudaGraphExecDestroy(g);
     if (len_event) cudaEventDestroy(len_event);
   }
 };
@@ -324,7 +330,7 @@ struct LaunchCfg {
   bool cooperative = false;     // every CTA resident at once (grid barriers)
 };
 // Every kernel of the library is launched here, and this is the only code that counts launches (vly_kernel_launch_count;
-// capture_steps derives vly_kv::graph_nodes from the count).  cudaLaunchKernelEx converts each argument to the kernel's
+// capture_steps derives StepGraphs::nodes from the count).  cudaLaunchKernelEx converts each argument to the kernel's
 // parameter type, as <<<>>> does.
 template <typename... KArgs, typename... Args>
 static int launch(vly_ctx* c, void (*kern)(KArgs...), const LaunchCfg& l, Args&&... args) {
@@ -1464,6 +1470,9 @@ static int launch_decode_attention(vly_ctx* c, DecAttnParams p, bool pdl, cudaSt
   return launch(c, decode_attention_v2_kernel, {dim3(p.B * p.nH, p.nsplit), dim3(128), 0, st, pdl, true}, p);
 }
 
+static int launch_logits_gemv(vly_ctx* c, vly_kv* kv, int b0, int nb, const bf16* x, long long ldx, long long* out_tokens, bool bump,
+                              bool pdl, cudaStream_t st);
+
 // Enqueue one decode step for batch rows [b0, b0+nb) of kv (nb <= 4).  Reads kv->cur_tokens, writes kv->cur_tokens.
 static int enqueue_decode_step(vly_ctx* c, vly_kv* kv, int b0, int nb, bool bump, cudaStream_t st) {
   const vly_config& g = c->cfg;
@@ -1507,22 +1516,25 @@ static int enqueue_decode_step(vly_ctx* c, vly_kv* kv, int b0, int nb, bool bump
       TRY(launch_gemv_ring<GEMV_RESIDUAL>(c, p, true, st));
     }
   }
-  {
-    GemvParams p = {};
-    p.N = V; p.K = H; p.B = nb; p.W = c->lm_head; p.x = x; p.eps = g.rms_norm_eps;
-    p.logits = kv->logits + (size_t)b0 * V;
-    p.part_val = kv->part_val + (size_t)b0 * c->num_sms;
-    p.part_idx = kv->part_idx + (size_t)b0 * c->num_sms;
-    p.counter = kv->counters + (size_t)kv->B * nH;
-    p.next_tokens = kv->cur_tokens + b0;
-    p.out_tokens = kv->gen_tokens + (size_t)b0 * kv->Smax;
-    p.out_stride = kv->Smax;
-    p.step = kv->d_step;
-    p.seq_len_rw = kv->d_len;
-    p.bump = bump ? 1 : 0;   // only the last batch group of a step advances the step / length counters
-    TRY(launch_gemv_ring<GEMV_LOGITS>(c, p, true, st));
-  }
-  return VLY_OK;
+  return launch_logits_gemv(c, kv, b0, nb, x, 0, kv->gen_tokens + (size_t)b0 * kv->Smax, bump, true, st);
+}
+
+// final RMSNorm (folded) + lm_head + arg-max for batch rows [b0, b0+nb) of kv (nb <= 4): x [nb, H] of row stride ldx (0 = H) ->
+// kv->logits and kv->cur_tokens, and column *d_step of out_tokens [nb, Smax] (nullptr: none).  bump: the last batch group of a
+// decode step, which advances the step / length counters.
+static int launch_logits_gemv(vly_ctx* c, vly_kv* kv, int b0, int nb, const bf16* x, long long ldx, long long* out_tokens, bool bump,
+                              bool pdl, cudaStream_t st) {
+  const vly_config& g = c->cfg;
+  GemvParams p = {};
+  p.N = g.vocab_size; p.K = g.hidden_size; p.B = nb; p.W = c->lm_head; p.x = x; p.ldx = ldx; p.eps = g.rms_norm_eps;
+  p.logits = kv->logits + (size_t)b0 * g.vocab_size;
+  p.part_val = kv->part_val + (size_t)b0 * c->num_sms;
+  p.part_idx = kv->part_idx + (size_t)b0 * c->num_sms;
+  p.counter = kv->counters + (size_t)kv->B * g.num_attention_heads;
+  p.next_tokens = kv->cur_tokens + b0;
+  p.out_tokens = out_tokens; p.out_stride = kv->Smax;
+  p.step = kv->d_step; p.seq_len_rw = kv->d_len; p.bump = bump ? 1 : 0;
+  return launch_gemv_ring<GEMV_LOGITS>(c, p, pdl, st);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1603,20 +1615,8 @@ extern "C" int vly_llama_prefill(vly_ctx* c, vly_kv* kv, const void* inputs_embe
     TRY(launch_gemm<EPI_RMS_F32>(c, 256, x, H, c->lm_head, H, p, st));
   }
   // last position only: final RMSNorm (folded) + lm_head GEMV + greedy argmax (model_worker.py:389-391)
-  for (int b0 = 0; b0 < B; b0 += 4) {
-    const int nb = (B - b0) < 4 ? (B - b0) : 4;
-    GemvParams p = {};
-    p.N = V; p.K = H; p.B = nb; p.W = c->lm_head; p.x = x + ((size_t)b0 * S + (S - 1)) * H; p.ldx = (long long)S * H;
-    p.eps = g.rms_norm_eps;
-    p.logits = kv->logits + (size_t)b0 * V;
-    p.part_val = kv->part_val + (size_t)b0 * c->num_sms;
-    p.part_idx = kv->part_idx + (size_t)b0 * c->num_sms;
-    p.counter = kv->counters + (size_t)kv->B * nH;
-    p.next_tokens = kv->cur_tokens + b0;
-    p.out_tokens = nullptr;
-    p.step = kv->d_step; p.seq_len_rw = kv->d_len; p.bump = 0;
-    TRY(launch_gemv_ring<GEMV_LOGITS>(c, p, false, st));
-  }
+  for (int b0 = 0; b0 < B; b0 += 4)
+    TRY(launch_logits_gemv(c, kv, b0, std::min(4, B - b0), x + ((size_t)b0 * S + (S - 1)) * H, (long long)S * H, nullptr, false, false, st));
   if (logits_mode == 1) CK(cudaMemcpyAsync(logits_dev, kv->logits, (size_t)B * V * 4, cudaMemcpyDeviceToDevice, st));
   if (next_tokens_dev) CK(cudaMemcpyAsync(next_tokens_dev, kv->cur_tokens, (size_t)B * 8, cudaMemcpyDeviceToDevice, st));
   kv->host_len = past + S;
@@ -1636,10 +1636,10 @@ extern "C" int vly_kv_debug_counters(vly_kv* kv, long long* host_out, int n) {
   return VLY_OK;
 }
 
-// the launch was planned by vly_kv_create (plan_decode_mega); filtered: sample_filter_kernel selects after the step
-static int launch_decode_mega(vly_ctx* c, vly_kv* kv, bool filtered, cudaStream_t st) {
+// the launch was planned by vly_kv_create (plan_decode_mega); select = false: the step ends with the logits, another kernel selects
+static int launch_decode_mega(vly_ctx* c, vly_kv* kv, bool select, cudaStream_t st) {
   StepParams p = kv->mega;
-  p.select = filtered ? 0 : 1;
+  p.select = select ? 1 : 0;
   LaunchCfg l = {dim3(c->num_sms), dim3(MegaCfg::THREADS), kv->mega_smem, st};
   l.cooperative = true;
   return with_bmax(kv->B, [&](auto bm) { return launch(c, decode_step_kernel<decltype(bm)::value>, l, p); });
@@ -1654,23 +1654,37 @@ static int launch_sample_filter(vly_ctx* c, const float* logits, int B, int V, S
                 out_stride, filter ? 1 : 0, per_op ? 1 : 0, keep_out);
 }
 
-// filtered: the step ends with sample_filter_kernel's filtered selection (set_sampling)
-static int enqueue_full_step(vly_ctx* c, vly_kv* kv, bool filtered, cudaStream_t st) {
-  if (kv->B <= 4) {
-    TRY(launch_decode_mega(c, kv, filtered, st));
-    if (filtered)
-      TRY(launch_sample_filter(c, kv->logits, kv->B, c->cfg.vocab_size, kv->d_sample, kv->d_len, kv->d_step, kv->cur_tokens,
-                               kv->gen_tokens, kv->Smax, true, false, nullptr, st));
-    return VLY_OK;
+// rows within groups of `group` take their parent's positions [*from_pos, *len) (kv_beam_reorder_kernel)
+static int launch_kv_beam_reorder(vly_ctx* c, vly_kv* kv, int group, const int* parent, const int* from_pos, const int* skip,
+                                  cudaStream_t st) {
+  const int nH = c->cfg.num_attention_heads, L = c->cfg.num_hidden_layers;
+  const size_t smem = (size_t)group * reorder_block_positions(group) * 256;
+  return launch(c, kv_beam_reorder_kernel, {dim3(L * 2 * (kv->B / group) * nH), dim3(kReorderThreads), smem, st}, kv->cache, kv->B,
+                nH, kv->Smax, group, parent, from_pos, (const int*)kv->d_len, skip);
+}
+
+static int launch_beam_step(vly_ctx* c, vly_kv* kv, int nb, const float* logits, cudaStream_t st) {
+  long long* fin = kv->beam_tok + (size_t)2 * kv->B * kv->Smax;
+  return launch(c, beam_step_kernel, {dim3(kv->B / nb), dim3(kBeamThreads), 0, st}, logits, c->cfg.vocab_size, kv->d_beam,
+                (long long*)kv->beam_tok, fin, kv->Smax, (const float*)kv->beam_div, (long long*)kv->cur_tokens, kv->d_sample);
+}
+
+// Enqueue one decode step of kv: the persistent kernel (B <= 4) or the per-op kernels per group of <= 4 rows, then what the
+// step kind selects with.  nb: beams per item (STEP_BEAM only).
+static int enqueue_step(vly_ctx* c, vly_kv* kv, StepKind kind, int nb, cudaStream_t st) {
+  const bool per_op = kv->B > 4;
+  if (!per_op) TRY(launch_decode_mega(c, kv, kind == STEP_TOKEN, st));
+  else
+    for (int b0 = 0; b0 < kv->B; b0 += 4) TRY(enqueue_decode_step(c, kv, b0, std::min(4, kv->B - b0), b0 + 4 >= kv->B, st));
+  if (kind == STEP_BEAM) {      // beam_step_kernel selects, the cache follows the parents
+    TRY(launch_beam_step(c, kv, nb, kv->logits, st));
+    return launch_kv_beam_reorder(c, kv, nb, kv->d_beam->parent, &kv->d_beam->prompt_len, &kv->d_beam->done, st);
   }
-  for (int b0 = 0; b0 < kv->B; b0 += 4) {
-    const int nb = (kv->B - b0) < 4 ? (kv->B - b0) : 4;
-    TRY(enqueue_decode_step(c, kv, b0, nb, b0 + 4 >= kv->B, st));
-  }
-  // per-op paths: sampling / eos bookkeeping as one more launch over the step's logits (returns at once when greedy)
-  if (kv->B <= kMaxSampleRows)
+  // a filtered token, or on the per-op path the sampling / eos bookkeeping (returns at once when greedy), is one more launch
+  // over the step's logits (a filter needs set_sampling, which allows at most kMaxSampleRows rows)
+  if (kind == STEP_FILTERED || (per_op && kv->B <= kMaxSampleRows))
     TRY(launch_sample_filter(c, kv->logits, kv->B, c->cfg.vocab_size, kv->d_sample, kv->d_len, kv->d_step, kv->cur_tokens,
-                             kv->gen_tokens, kv->Smax, filtered, true, nullptr, st));
+                             kv->gen_tokens, kv->Smax, kind == STEP_FILTERED, per_op, nullptr, st));
   return VLY_OK;
 }
 
@@ -1684,12 +1698,13 @@ __global__ void set_sample_state_kernel(SampleState* s, const SampleState r, int
   if (reset_done && threadIdx.x < kMaxSampleRows) s->done[threadIdx.x] = 0;
 }
 
-// sampling == nullptr: plain greedy, no stop token (skipped when the device state already says so)
-static int set_sampling(vly_ctx* c, vly_kv* kv, const vly_sampling* sp, bool reset_done, cudaStream_t st) {
+// sampling == nullptr: plain greedy, no stop token (skipped when the device state already says so, unless `force`: a beam
+// search starts from that state and leaves all_done raised, so it always resets it and leaves it dirty)
+static int set_sampling(vly_ctx* c, vly_kv* kv, const vly_sampling* sp, bool reset_done, cudaStream_t st, bool force = false) {
   SampleState r = {};
   kv->filtered = false;
   if (!sp) {
-    if (!kv->sample_dirty) return VLY_OK;
+    if (!kv->sample_dirty && !force) return VLY_OK;
     reset_done = true;
   } else {
     if (kv->B > kMaxSampleRows) return fail(VLY_ERR_INVALID, "sampling / eos bookkeeping supports at most %d sequences per cache", kMaxSampleRows);
@@ -1704,7 +1719,7 @@ static int set_sampling(vly_ctx* c, vly_kv* kv, const vly_sampling* sp, bool res
     // the filters apply only when sampling (HF ignores its warpers when it does not sample)
     kv->filtered = on && (sp->top_k > 0 || (sp->top_p > 0.f && sp->top_p < 1.f));
   }
-  kv->sample_dirty = sp != nullptr;
+  kv->sample_dirty = sp != nullptr || force;
   return launch(c, set_sample_state_kernel, {dim3(1), dim3(64), 0, st}, kv->d_sample, r, reset_done ? 1 : 0);
 }
 
@@ -1730,12 +1745,38 @@ static int capture_steps(vly_ctx* c, int n, F&& enqueue_step, cudaGraphExec_t* o
   if (e2 != cudaSuccess) return fail(VLY_ERR_CUDA, "cudaGraphInstantiate: %s", cudaGetErrorString(e2));
   return VLY_OK;
 }
-static int build_graph(vly_ctx* c, vly_kv* kv, bool filtered) {
-  cudaGraphExec_t* g = kv->graph[filtered];
-  if (g[0]) return VLY_OK;
-  auto step = [&](cudaStream_t st) { return enqueue_full_step(c, kv, filtered, st); };
-  TRY(capture_steps(c, 1, step, &g[0], &kv->graph_nodes[filtered]));
-  TRY(capture_steps(c, kGraphSteps, step, &g[1], &kv->graph_nodes[filtered]));
+// Run n decode steps of one kind on st as replays of its kGraphSteps-step graph, then of its 1-step graph; each replayed step
+// counts its kernels.  VLY_NO_GRAPH=1 (profiling aid): eager launches instead.
+static int run_steps(vly_ctx* c, vly_kv* kv, StepKind kind, int nb, int n, cudaStream_t st) {
+  static const bool no_graph = getenv("VLY_NO_GRAPH") != nullptr;
+  auto step = [&](cudaStream_t s) { return enqueue_step(c, kv, kind, nb, s); };
+  if (no_graph) {
+    for (int i = 0; i < n; ++i) TRY(step(st));
+    return VLY_OK;
+  }
+  StepGraphs& g = kv->graphs[kind];
+  if (!g.many || g.nb != nb) {
+    g.reset();
+    TRY(capture_steps(c, 1, step, &g.one, &g.nodes));
+    TRY(capture_steps(c, kGraphSteps, step, &g.many, &g.nodes));
+    g.nb = nb;
+  }
+  for (int i = 0; i < n;) {
+    if (n - i >= kGraphSteps) { CK(cudaGraphLaunch(g.many, st)); i += kGraphSteps; }
+    else { CK(cudaGraphLaunch(g.one, st)); ++i; }
+  }
+  c->launches += (int64_t)n * g.nodes;
+  return VLY_OK;
+}
+
+// the request advanced the cache by n positions, or fewer when the device may have stopped early (a stop id, the end of a beam
+// search): then the device's length is copied back behind the request, and sync_len reads it on the cache's next use
+static int finish_request(vly_kv* kv, int n, bool may_stop_early, cudaStream_t st) {
+  kv->host_len += n;
+  if (!may_stop_early) return VLY_OK;
+  CK(cudaMemcpyAsync(kv->h_len, kv->d_len, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaEventRecord(kv->len_event, st));
+  kv->len_dirty = true;
   return VLY_OK;
 }
 
@@ -1769,33 +1810,18 @@ static int generate_impl(vly_ctx* c, vly_kv* kv, const int64_t* first_tokens, in
   if (kv->host_len + n_steps > kv->Smax) return fail(VLY_ERR_INVALID, "vly_generate: %d cached + %d steps exceed the cache capacity %d", kv->host_len, n_steps, kv->Smax);
   CK(cudaSetDevice(c->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  static const bool no_graph = getenv("VLY_NO_GRAPH") != nullptr;   // profiling aid: eager launches instead of graph replay
   // with a sampling struct the eos flags raised by vly_sample_logits (the first token) are kept; greedy starts clean
   TRY(set_sampling(c, kv, sp, false, st));
-  const bool filtered = kv->filtered;
-  if (!no_graph) TRY(build_graph(c, kv, filtered));
-  cudaGraphExec_t one = kv->graph[filtered][0], many = kv->graph[filtered][1];
   CK(cudaMemcpyAsync(kv->cur_tokens, first_tokens, (size_t)kv->B * 8, cudaMemcpyDeviceToDevice, st));
   CK(cudaMemsetAsync(kv->d_step, 0, 4, st));
   if (steps_done_dev) CK(cudaMemsetAsync(&kv->d_sample->steps_valid, 0, 4, st));
-  for (int i = 0; i < n_steps;) {
-    if (no_graph) { TRY(enqueue_full_step(c, kv, filtered, st)); ++i; }
-    else if (many && n_steps - i >= kGraphSteps) { CK(cudaGraphLaunch(many, st)); i += kGraphSteps; }
-    else { CK(cudaGraphLaunch(one, st)); ++i; }
-  }
-  if (!no_graph) c->launches += (int64_t)n_steps * kv->graph_nodes[filtered];
+  TRY(run_steps(c, kv, kv->filtered ? STEP_FILTERED : STEP_TOKEN, 0, n_steps, st));
   if (out_tokens)
     CK(cudaMemcpy2DAsync(out_tokens, (size_t)n_steps * 8, kv->gen_tokens, (size_t)kv->Smax * 8, (size_t)n_steps * 8, kv->B,
                          cudaMemcpyDeviceToDevice, st));
-  if (steps_done_dev)      // (zeroed below, before the first step)
+  if (steps_done_dev)      // (zeroed above, before the first step)
     CK(cudaMemcpyAsync(steps_done_dev, &kv->d_sample->steps_valid, 4, cudaMemcpyDeviceToDevice, st));
-  kv->host_len += n_steps;
-  if (sp && (sp->eos_token_id >= 0 || sp->stop_token_id >= 0)) {     // the loop may have stopped early: the device holds the true length
-    CK(cudaMemcpyAsync(kv->h_len, kv->d_len, 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaEventRecord(kv->len_event, st));
-    kv->len_dirty = true;
-  }
-  return VLY_OK;
+  return finish_request(kv, n_steps, sp && (sp->eos_token_id >= 0 || sp->stop_token_id >= 0), st);
 }
 
 extern "C" int vly_llama_decode(vly_ctx* c, vly_kv* kv, const int64_t* tokens, int64_t* next_tokens, void* logits_dev, void* stream) {
@@ -1805,16 +1831,13 @@ extern "C" int vly_llama_decode(vly_ctx* c, vly_kv* kv, const int64_t* tokens, i
   if (kv->host_len + 1 > kv->Smax) return fail(VLY_ERR_INVALID, "vly_llama_decode: cache full (%d)", kv->Smax);
   CK(cudaSetDevice(c->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  TRY(build_graph(c, kv, false));
   TRY(set_sampling(c, kv, nullptr, true, st));
   CK(cudaMemcpyAsync(kv->cur_tokens, tokens, (size_t)kv->B * 8, cudaMemcpyDeviceToDevice, st));
   CK(cudaMemsetAsync(kv->d_step, 0, 4, st));
-  CK(cudaGraphLaunch(kv->graph[0][0], st));
-  c->launches += kv->graph_nodes[0];
+  TRY(run_steps(c, kv, STEP_TOKEN, 0, 1, st));
   if (next_tokens) CK(cudaMemcpyAsync(next_tokens, kv->cur_tokens, (size_t)kv->B * 8, cudaMemcpyDeviceToDevice, st));
   if (logits_dev) CK(cudaMemcpyAsync(logits_dev, kv->logits, (size_t)kv->B * c->cfg.vocab_size * 4, cudaMemcpyDeviceToDevice, st));
-  kv->host_len += 1;
-  return VLY_OK;
+  return finish_request(kv, 1, false, st);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1827,33 +1850,6 @@ static int ensure_beam_buffers(vly_kv* kv) {
   TRY(kv->beam_div.alloc((size_t)kv->Smax * sizeof(float)));
   TRY(kv->beam_from.alloc(sizeof(int)));
   return VLY_OK;
-}
-
-// rows within groups of `group` take their parent's positions [*from_pos, *len) (kv_beam_reorder_kernel)
-static int launch_kv_beam_reorder(vly_ctx* c, vly_kv* kv, int group, const int* parent, const int* from_pos, const int* skip,
-                                  cudaStream_t st) {
-  const int nH = c->cfg.num_attention_heads, L = c->cfg.num_hidden_layers;
-  const size_t smem = (size_t)group * reorder_block_positions(group) * 256;
-  return launch(c, kv_beam_reorder_kernel, {dim3(L * 2 * (kv->B / group) * nH), dim3(kReorderThreads), smem, st}, kv->cache, kv->B,
-                nH, kv->Smax, group, parent, from_pos, (const int*)kv->d_len, skip);
-}
-
-static int launch_beam_step(vly_ctx* c, vly_kv* kv, int nb, const float* logits, cudaStream_t st) {
-  long long* fin = kv->beam_tok + (size_t)2 * kv->B * kv->Smax;
-  return launch(c, beam_step_kernel, {dim3(kv->B / nb), dim3(kBeamThreads), 0, st}, logits, c->cfg.vocab_size, kv->d_beam,
-                (long long*)kv->beam_tok, fin, kv->Smax, (const float*)kv->beam_div, (long long*)kv->cur_tokens, kv->d_sample);
-}
-
-// one decode step of a beam request: the step writes the logits (select = 0), beam_step_kernel selects, the cache follows the
-// parents
-static int enqueue_beam_step(vly_ctx* c, vly_kv* kv, int nb, cudaStream_t st) {
-  if (kv->B <= 4) {
-    TRY(launch_decode_mega(c, kv, true, st));
-  } else {
-    for (int b0 = 0; b0 < kv->B; b0 += 4) TRY(enqueue_decode_step(c, kv, b0, std::min(4, kv->B - b0), b0 + 4 >= kv->B, st));
-  }
-  TRY(launch_beam_step(c, kv, nb, kv->logits, st));
-  return launch_kv_beam_reorder(c, kv, nb, kv->d_beam->parent, &kv->d_beam->prompt_len, &kv->d_beam->done, st);
 }
 
 extern "C" int vly_beam_search(vly_ctx* c, vly_kv* kv, const vly_beam* bp, const float* first_logits, int prompt_len, int n_steps,
@@ -1873,38 +1869,18 @@ extern "C" int vly_beam_search(vly_ctx* c, vly_kv* kv, const vly_beam* bp, const
   CK(cudaSetDevice(c->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   TRY(ensure_beam_buffers(kv));
-  if (kv->beam_graph_nb != nb) {
-    for (cudaGraphExec_t& g : kv->beam_graph) {
-      if (g) cudaGraphExecDestroy(g);
-      g = nullptr;
-    }
-    auto step = [&](cudaStream_t s) { return enqueue_beam_step(c, kv, nb, s); };
-    TRY(capture_steps(c, 1, step, &kv->beam_graph[0], &kv->beam_nodes));
-    TRY(capture_steps(c, kGraphSteps, step, &kv->beam_graph[1], &kv->beam_nodes));
-    kv->beam_graph_nb = nb;
-  }
   // plain selection state: the decode steps write logits only, and exit once beam_step_kernel raises all_done
-  kv->filtered = false;
-  kv->sample_dirty = true;            // (all_done stays raised after the search: the next request resets the state)
-  TRY(launch(c, set_sample_state_kernel, {dim3(1), dim3(64), 0, st}, kv->d_sample, SampleState{}, 1));
+  TRY(set_sampling(c, kv, nullptr, true, st, true));
   TRY(launch(c, beam_init_kernel, {dim3(1), dim3(256), 0, st}, kv->d_beam, kv->B, nb, n_steps, prompt_len, (int)bp->early_stopping,
              bp->length_penalty, (long long)(bp->eos_token_id < 0 ? -1 : bp->eos_token_id), (float*)kv->beam_div));
   TRY(launch_beam_step(c, kv, nb, first_logits, st));
   CK(cudaMemsetAsync(kv->d_step, 0, 4, st));
-  for (int i = 0; i < n_steps - 1;) {
-    if (n_steps - 1 - i >= kGraphSteps) { CK(cudaGraphLaunch(kv->beam_graph[1], st)); i += kGraphSteps; }
-    else { CK(cudaGraphLaunch(kv->beam_graph[0], st)); ++i; }
-  }
-  c->launches += (int64_t)(n_steps - 1) * kv->beam_nodes;
+  TRY(run_steps(c, kv, STEP_BEAM, nb, n_steps - 1, st));
   const long long* fin = kv->beam_tok + (size_t)2 * kv->B * kv->Smax;
   TRY(launch(c, beam_output_kernel, {dim3(kv->B / nb * nrs), dim3(256), 0, st}, (const BeamState*)kv->d_beam, fin, kv->Smax, kv->B, nrs,
              n_steps, (long long)bp->pad_token_id, (long long*)seq_out, scores_out, gen_len_out));
-  // the steps after the end of the search did not advance the cache: the device holds its length
-  kv->host_len += n_steps - 1;
-  CK(cudaMemcpyAsync(kv->h_len, kv->d_len, 4, cudaMemcpyDeviceToHost, st));
-  CK(cudaEventRecord(kv->len_event, st));
-  kv->len_dirty = true;
-  return VLY_OK;
+  // the steps after the end of the search did not advance the cache
+  return finish_request(kv, n_steps - 1, true, st);
 }
 
 extern "C" int vly_kv_beam_reorder(vly_ctx* c, vly_kv* kv, const int32_t* parent_rows, int from_pos, void* stream) {

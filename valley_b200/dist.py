@@ -159,12 +159,12 @@ def generate_sharded(model, input_ids: torch.Tensor, local_pixels: torch.Tensor,
                                                                     frame_features=mine, n_frames=n_frames)
     if fused is not None:
         fused.release()                                       # the gather buffer has been consumed (stream order)
-    cache = model._borrow_cache(B)
+    cache = model.new_cache(B)
     try:
         S = input_ids.shape[1]
         out = model._generate_with_cache(cache, input_ids, embeds, max_new_tokens, False, 1.0, None, None)[:, S:]
     finally:
-        model._return_cache(cache)
+        cache.release()
     if fused is not None:
         fused.check()          # a timed-out gather of an EARLIER request is reported here at the latest (pinned flag, no sync)
     return out

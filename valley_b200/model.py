@@ -639,15 +639,6 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
     def new_cache(self, batch: int, max_seq: Optional[int] = None) -> ValleyKVCache:
         return ValleyKVCache(self, batch, max_seq or self.config.max_position_embeddings)
 
-    def _borrow_cache(self, batch: int) -> ValleyKVCache:
-        """generate() recycles its KV-cache handles (and the CUDA graphs captured on them) through the model's handle pool
-        instead of paying a multi-GB cudaMalloc + graph capture per request.  The pool is per model instance and
-        lock-protected (model_worker.py:467-474 calls the model from several threads)."""
-        return self.new_cache(batch)
-
-    def _return_cache(self, c: ValleyKVCache):
-        c.release()
-
     def _prefill(self, cache: ValleyKVCache, embeds: torch.Tensor, logits_mode: int):
         B, S, _ = embeds.shape
         V = self.config.vocab_size
@@ -758,26 +749,34 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
                                        num_return_sequences, length_penalty, early_stopping, **kw)
         greedy = (not do_sample) or temperature < 1e-4
         filters = {} if greedy else dict(zip(("top_k", "top_p"), sampling_filters(top_k, top_p)))
-        room = self.config.max_position_embeddings - S
-        n_new = max(0, min(max_new_tokens, room))
+        n_new, eos_token_id, pad_token_id, attention_mask = self._generation_defaults(input_ids, max_new_tokens, eos_token_id, kw)
         if n_new == 0:
             return input_ids.to(self.device)
-        if eos_token_id is _UNSET:
-            eos_token_id = getattr(self.config, "eos_token_id", None)
-        pad_token_id = kw.get("pad_token_id", getattr(self.config, "pad_token_id", None))
-        attention_mask = kw.get("attention_mask")
-        if attention_mask is None and pad_token_id is not None and (eos_token_id is None or pad_token_id != eos_token_id):
-            is_pad = input_ids == pad_token_id
-            if bool(is_pad.any()):
-                attention_mask = (~is_pad).to(torch.int64)
         _, _, _, embeds, _ = self.prepare_inputs_labels_for_multimodal(input_ids, None, None, None, images)
-        cache = self._borrow_cache(B)
+        cache = self.new_cache(B)
         try:
             cache.set_attention_mask(attention_mask, S)
             return self._generate_with_cache(cache, input_ids, embeds, n_new, do_sample, temperature, stopping_criteria, eos_token_id,
                                              pad_token_id, **filters)
         finally:
-            self._return_cache(cache)
+            cache.release()
+
+    def _generation_defaults(self, input_ids, max_new_tokens, eos_token_id, kw):
+        """(n_new, eos_token_id, pad_token_id, attention_mask) of a generate() request, with the HF defaults generate() describes:
+        at most the tokens the context has room for, eos and pad from the config, pad falling back to eos, and the attention
+        mask inferred from pad tokens in the prompt (pad != eos)."""
+        n_new = max(0, min(max_new_tokens, self.config.max_position_embeddings - input_ids.shape[1]))
+        if eos_token_id is _UNSET:
+            eos_token_id = getattr(self.config, "eos_token_id", None)
+        pad_token_id = kw.get("pad_token_id", getattr(self.config, "pad_token_id", None))
+        if pad_token_id is None:
+            pad_token_id = eos_token_id                       # HF generate: pad defaults to eos
+        attention_mask = kw.get("attention_mask")
+        if attention_mask is None and pad_token_id is not None and pad_token_id != eos_token_id:
+            is_pad = input_ids == pad_token_id
+            if bool(is_pad.any()):
+                attention_mask = (~is_pad).to(torch.int64)
+        return n_new, eos_token_id, pad_token_id, attention_mask
 
     def _generate_with_cache(self, cache, input_ids, embeds, n_new, do_sample, temperature, stopping_criteria, eos_token_id,
                              pad_token_id=None, top_k=0, top_p=1.0):
@@ -851,27 +850,17 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
             raise ValueError(f"`early_stopping` must be a boolean or 'never', but is {early_stopping}.")
         B, S = input_ids.shape
         nb = num_beams
-        n_new = max(0, min(max_new_tokens, self.config.max_position_embeddings - S))
+        n_new, eos_token_id, pad_token_id, attention_mask = self._generation_defaults(input_ids, max_new_tokens, eos_token_id, kw)
         ids_dev = input_ids.to(self.device, torch.int64)
         if n_new == 0:
             return _repeat_rows(ids_dev, num_return_sequences)
-        if eos_token_id is _UNSET:
-            eos_token_id = getattr(self.config, "eos_token_id", None)
-        pad_token_id = kw.get("pad_token_id", getattr(self.config, "pad_token_id", None))
-        if pad_token_id is None and eos_token_id is not None:
-            pad_token_id = eos_token_id                       # HF generate: pad defaults to eos
-        attention_mask = kw.get("attention_mask")
-        if attention_mask is None and pad_token_id is not None and (eos_token_id is None or pad_token_id != eos_token_id):
-            is_pad = input_ids == pad_token_id
-            if bool(is_pad.any()):
-                attention_mask = (~is_pad).to(torch.int64)
         fill = _beam.output_fill_value(pad_token_id, eos_token_id)
         _, _, _, embeds, _ = self.prepare_inputs_labels_for_multimodal(input_ids, None, None, None, images)
         embeds = _repeat_rows(embeds, nb)
         ids_rep = _repeat_rows(ids_dev, nb)
         if attention_mask is not None:
             attention_mask = _repeat_rows(attention_mask, nb)
-        cache = self._borrow_cache(B * nb)
+        cache = self.new_cache(B * nb)
         try:
             cache.set_attention_mask(attention_mask, S)
             logits, _ = self._prefill(cache, embeds, 1)
@@ -908,7 +897,7 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
             out, self.last_beam_scores = bs.result(num_return_sequences)
             return out
         finally:
-            self._return_cache(cache)
+            cache.release()
 
     # ---------------- prompt helpers (pure string logic; valley_model.py:381-422) ----------------
     def build_inputs(self, tokenizer, messages):

@@ -80,7 +80,7 @@ def generate_stream(model, tokenizer, params: Dict, *, context_len: int = 2048, 
     if max_new_tokens <= 0:
         return
     _, _, _, embeds, _ = model.prepare_inputs_labels_for_multimodal(ids, None, None, None, images)
-    cache = model._borrow_cache(1)
+    cache = model.new_cache(1)
     try:
         logits, _ = model._prefill(cache, embeds, 1)
         sp = VlySampling(temperature if temperature >= 1e-4 else 0.0, int(torch.randint(0, 2 ** 62, (1,)).item()),
@@ -117,4 +117,4 @@ def generate_stream(model, tokenizer, params: Dict, *, context_len: int = 2048, 
                 continue
             tok.copy_(chunk[0, n - 1:n])
     finally:
-        model._return_cache(cache)
+        cache.release()
