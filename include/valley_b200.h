@@ -207,6 +207,24 @@ typedef struct {
   int64_t stop_token_id;     /* -1: none; a second id that ends a row: the worker's single-token stop string (model_worker.py:355-360, :396-397) */
   int32_t top_k;             /* <= 0: off */
   float top_p;               /* off unless 0 < top_p < 1 */
+  /* Stop strings: transformers' StopStringCriteria (generate(stop_strings=...)), matched on the device after each token is
+   * selected.  A row whose text -- the concatenation of its tokens' clean strings -- ends with a stop string, the last
+   * characters inside the newest token, is finished; so is a row that emits a token of pause_bits.  A finished row emits
+   * pad_token_id afterwards only when eos_token_id or stop_token_id is set (HF pads only with an eos criterion); the remaining
+   * steps are skipped once every row has finished.  The tables are built by valley_b200/stop_strings.py (stop_tables); V is
+   * the context's vocab_size.  Every host array is copied before the call returns.  At most 64 rows.  Zero: no stop strings. */
+  int32_t n_stop_strings;          /* 0..8 */
+  const int32_t* stop_lens;        /* host [n_stop_strings]: characters of each stop string, 1..64 */
+  const uint64_t* stop_masks;      /* host [n_stop_strings][V][2]: per token, the end mask (bit L-1: the token can be the last one
+                                    * with the last L characters of the string inside it, trailing characters allowed) and the
+                                    * position mask (bit p: the token fits with its end p characters before the string's end) */
+  const int32_t* stop_token_lens;  /* host [V]: each token's clean-string length */
+  const uint32_t* pause_bits;      /* host [ceil(V / 32)] bit set of tokens that finish a row as a match does, or NULL */
+  const int64_t* stop_tail;        /* host [B][stop_tail_len]: each row's last tokens before its first selected token */
+  int32_t stop_tail_len;           /* 0..63 */
+  int32_t stop_restart;            /* vly_generate: 1 = start the matcher here (upload the tables, seed the rows from stop_tail
+                                    * and clear the finished flags); 0 = continue the request vly_sample_logits started.
+                                    * vly_sample_logits always starts it. */
 } vly_sampling;
 
 /* the first generated token: select from the prefill's last-position logits [B,V] fp32 (vly_llama_prefill logits_mode 1);
@@ -271,6 +289,11 @@ int vly_test_vit_attention(vly_ctx* ctx, const void* qkv_dev, int n_frames, void
  * computed by the same device routine the decode loop selects with.  temperature > 0; top_k / top_p as in vly_sampling. */
 int vly_test_sample_filter(vly_ctx* ctx, const float* logits_dev, int B, int V, float temperature, int top_k, float top_p,
                            uint8_t* keep_out_dev, void* stream);
+/* the stop-string matcher of vly_sampling alone: with the stop-string fields of `sampling` (tables over a vocabulary of V
+ * tokens; the tail and pause fields are not used), out_dev[b] (uint8) = 1 when row b of tokens_dev [B, n] int64, read as a
+ * row whose newest token is the last, matches.  B <= 64.  Synchronises the stream. */
+int vly_test_stop_strings(vly_ctx* ctx, const vly_sampling* sampling, int V, const int64_t* tokens_dev, int B, int n,
+                          uint8_t* out_dev, void* stream);
 /* one weight-streaming GEMV of the per-op decode step, through the launcher the step uses: y[b,n] = sum_k x[b,k] W[n,k] with
  * W [N,K] bf16, x [B,K] bf16 of row stride ldx (0 = K), B <= 4, K and ldx multiples of 8, W and x 16-byte aligned.  rstd[b] = 1/sqrt(mean_k x[b,k]^2 + eps)
  * (the RMSNorm whose gamma is folded into W).  mode:

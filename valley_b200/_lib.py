@@ -35,10 +35,40 @@ class VlyTokens(C.Structure):
 
 class VlySampling(C.Structure):
     _fields_ = [("temperature", C.c_float), ("seed", C.c_uint64), ("eos_token_id", C.c_int64), ("pad_token_id", C.c_int64),
-                ("stop_token_id", C.c_int64), ("top_k", C.c_int32), ("top_p", C.c_float)]
+                ("stop_token_id", C.c_int64), ("top_k", C.c_int32), ("top_p", C.c_float),
+                ("n_stop_strings", C.c_int32), ("stop_lens", C.POINTER(C.c_int32)), ("stop_masks", C.POINTER(C.c_uint64)),
+                ("stop_token_lens", C.POINTER(C.c_int32)), ("pause_bits", C.POINTER(C.c_uint32)),
+                ("stop_tail", C.POINTER(C.c_int64)), ("stop_tail_len", C.c_int32), ("stop_restart", C.c_int32)]
 
     def __init__(self, temperature=0.0, seed=0, eos_token_id=-1, pad_token_id=0, stop_token_id=-1, top_k=0, top_p=1.0):
         super().__init__(temperature, seed, eos_token_id, pad_token_id, stop_token_id, top_k, top_p)
+        self._keep = ()
+
+    def set_stop_strings(self, tables, tail=None, pause=None, restart=False):
+        """Point the stop-string fields at ``tables`` (``stop_strings.StopTables``), the rows' last tokens before the first
+        selected one (``tail`` [B, <= 63] int64 CPU, or None) and the pause bit set (uint32 CPU, or None).  The arrays are
+        kept alive with the struct; the library copies them during the call."""
+        import numpy as np
+        lens = np.ascontiguousarray(tables.lens, dtype=np.int32)
+        masks = np.ascontiguousarray(tables.masks, dtype=np.uint64)
+        tok = np.ascontiguousarray(tables.token_lens, dtype=np.int32)
+        keep = [lens, masks, tok]
+        self.n_stop_strings = len(lens)
+        self.stop_lens = lens.ctypes.data_as(C.POINTER(C.c_int32))
+        self.stop_masks = masks.ctypes.data_as(C.POINTER(C.c_uint64))
+        self.stop_token_lens = tok.ctypes.data_as(C.POINTER(C.c_int32))
+        if pause is not None:
+            pause = np.ascontiguousarray(pause, dtype=np.uint32)
+            keep.append(pause)
+            self.pause_bits = pause.ctypes.data_as(C.POINTER(C.c_uint32))
+        if tail is not None and tail.shape[1] > 0:
+            t = np.ascontiguousarray(np.asarray(tail, dtype=np.int64))
+            keep.append(t)
+            self.stop_tail = t.ctypes.data_as(C.POINTER(C.c_int64))
+            self.stop_tail_len = t.shape[1]
+        self.stop_restart = 1 if restart else 0
+        self._keep = tuple(keep)
+        return self
 
 
 class VlyBeam(C.Structure):
@@ -97,7 +127,8 @@ SIGNATURES = {
     "vly_test_gemm": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp]),
     "vly_test_vit_attention": (_i, [_vp, _vp, _i, _vp, _vp]),
     "vly_test_sample_filter": (_i, [_vp, _vp, _i, _i, C.c_float, _i, C.c_float, _vp, _vp]),
-    "vly_test_gemv": (_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i64, C.c_float, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
+    "vly_test_stop_strings": (_i, [_vp, _p(VlySampling), _i, _vp, _i, _i, _vp, _vp]),
+    "vly_test_gemv":(_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i64, C.c_float, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     "vly_test_decode_attention": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
 }
 

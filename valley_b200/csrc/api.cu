@@ -242,6 +242,11 @@ struct vly_kv {
   Owned<long long> beam_tok;
   Owned<float> beam_div;
   Owned<int> beam_from;               // vly_kv_beam_reorder's first position
+  // stop strings (set_sampling), allocated on the cache's first stop-string request: the tables and the per-row token rings
+  // on the device (stop_layout), and the pinned copy they are uploaded from (stop_event: the last upload has read it)
+  Owned<uint8_t> stop_buf, stop_stage;
+  cudaEvent_t stop_event = nullptr;
+  bool stop_ready = false;            // the running request has stop strings, and its tables and rings are on the device
   StepGraphs graphs[kStepKinds];      // (declared after the buffers they refer to: destroyed before them)
   size_t layer_stride() const { return (size_t)2 * B * ctx->cfg.num_attention_heads * Smax * 128; }
   bf16* k_layer(int l) const { return cache + (size_t)l * layer_stride(); }
@@ -249,6 +254,7 @@ struct vly_kv {
 
   ~vly_kv() {
     if (len_event) cudaEventDestroy(len_event);
+    if (stop_event) cudaEventDestroy(stop_event);
   }
 };
 
@@ -1691,22 +1697,110 @@ static int enqueue_step(vly_ctx* c, vly_kv* kv, StepKind kind, int nb, cudaStrea
 // ---- token selection state ----
 __global__ void set_sample_state_kernel(SampleState* s, const SampleState r, int reset_done) {
   if (threadIdx.x == 0) {
-    s->temperature = r.temperature; s->inv_temp = r.inv_temp; s->enabled = r.enabled; s->top_k = r.top_k; s->top_p = r.top_p;
-    s->seed_lo = r.seed_lo; s->seed_hi = r.seed_hi; s->eos = r.eos; s->pad = r.pad; s->stop2 = r.stop2;
+    s->temperature = r.temperature; s->inv_temp = r.inv_temp; s->enabled = r.enabled; s->filter = r.filter; s->top_k = r.top_k;
+    s->top_p = r.top_p; s->seed_lo = r.seed_lo; s->seed_hi = r.seed_hi; s->eos = r.eos; s->pad = r.pad; s->stop2 = r.stop2;
+    s->n_stop = r.n_stop; s->stop_walk = r.stop_walk; s->stop_masks = r.stop_masks; s->tok_len = r.tok_len; s->pause = r.pause;
+    s->ring = r.ring;
     if (reset_done) { s->all_done = 0; s->steps_valid = 0; }
   }
-  if (reset_done && threadIdx.x < kMaxSampleRows) s->done[threadIdx.x] = 0;
+  if (threadIdx.x < kMaxStopStrings) s->stop_len[threadIdx.x] = r.stop_len[threadIdx.x];
+  if (reset_done && threadIdx.x < kMaxSampleRows) { s->done[threadIdx.x] = 0; s->ring_n[threadIdx.x] = r.ring_n[threadIdx.x]; }
+}
+
+// ---- stop strings ----
+// kv->stop_buf: [kMaxStopStrings][V] ulonglong2 masks | [V] uint8 token lengths | [ceil(V/32)] uint32 pause bits |
+// [kMaxSampleRows][kStopRing] int32 rings.  stop_stage (pinned) has the same layout.
+struct StopLayout {
+  size_t lens, pause, ring, bytes;
+  explicit StopLayout(int V) {
+    auto up = [](size_t x) { return (x + 255) & ~size_t(255); };
+    lens = (size_t)kMaxStopStrings * V * sizeof(ulonglong2);
+    pause = up(lens + V);
+    ring = up(pause + (size_t)cdiv(V, 32) * 4);
+    bytes = ring + (size_t)kMaxSampleRows * kStopRing * 4;
+  }
+};
+
+static int check_stop_tables(const vly_sampling* sp, int B, const char* who) {
+  const int n = sp->n_stop_strings;
+  if (n < 0 || n > kMaxStopStrings || !sp->stop_lens || !sp->stop_masks || !sp->stop_token_lens)
+    return fail(VLY_ERR_INVALID, "%s: n_stop_strings %d must be in [1, %d] with stop_lens, stop_masks and stop_token_lens", who, n, kMaxStopStrings);
+  for (int i = 0; i < n; ++i)
+    if (sp->stop_lens[i] < 1 || sp->stop_lens[i] > kMaxStopChars)
+      return fail(VLY_ERR_INVALID, "%s: stop string %d has %d characters (1..%d on the device)", who, i, sp->stop_lens[i], kMaxStopChars);
+  if (sp->stop_tail_len < 0 || sp->stop_tail_len >= kStopRing || (sp->stop_tail_len > 0 && !sp->stop_tail))
+    return fail(VLY_ERR_INVALID, "%s: stop_tail_len %d must be in [0, %d) with a stop_tail", who, sp->stop_tail_len, kStopRing);
+  if (B > kMaxSampleRows) return fail(VLY_ERR_INVALID, "%s: stop strings support at most %d rows (%d)", who, kMaxSampleRows, B);
+  return VLY_OK;
+}
+
+// The SampleState fields of sp's stop strings over the device buffer `dev` (StopLayout); ring_n from the tail length.
+static void stop_state(const vly_sampling* sp, uint8_t* dev, int V, SampleState& r) {
+  const StopLayout l(V);
+  r.n_stop = sp->n_stop_strings;
+  r.stop_walk = 0;
+  for (int i = 0; i < r.n_stop; ++i) {
+    r.stop_len[i] = sp->stop_lens[i];
+    r.stop_walk = std::max(r.stop_walk, sp->stop_lens[i]);
+  }
+  r.stop_masks = (const ulonglong2*)dev;
+  r.tok_len = dev + l.lens;
+  r.pause = sp->pause_bits ? (const uint32_t*)(dev + l.pause) : nullptr;
+  r.ring = (int*)(dev + l.ring);
+  for (int b = 0; b < kMaxSampleRows; ++b) r.ring_n[b] = sp->stop_tail_len;
+}
+
+// Uploads sp's tables and each row's tail (seeding its ring) to `dev` through the pinned `stage`; every host array is read
+// before this returns.  The wait on `ev` only blocks when the previous upload from `stage` has not run yet.
+static int upload_stop_tables(const vly_sampling* sp, int B, int V, uint8_t* dev, uint8_t* stage, cudaEvent_t ev, cudaStream_t st) {
+  const StopLayout l(V);
+  const int n = sp->n_stop_strings, tail = sp->stop_tail_len;
+  CK(cudaEventSynchronize(ev));
+  const size_t mask_bytes = (size_t)n * V * sizeof(ulonglong2);
+  memcpy(stage, sp->stop_masks, mask_bytes);
+  for (int t = 0; t < V; ++t) stage[l.lens + t] = (uint8_t)std::min<int32_t>(sp->stop_token_lens[t], 255);
+  const size_t pause_bytes = sp->pause_bits ? (size_t)cdiv(V, 32) * 4 : 0;
+  if (pause_bytes) memcpy(stage + l.pause, sp->pause_bits, pause_bytes);
+  int* ring = (int*)(stage + l.ring);
+  for (int b = 0; b < B; ++b)
+    for (int j = 0; j < tail; ++j) ring[b * kStopRing + j] = (int)sp->stop_tail[(size_t)b * tail + j];
+  CK(cudaMemcpyAsync(dev, stage, mask_bytes, cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(dev + l.lens, stage + l.lens, (size_t)V, cudaMemcpyHostToDevice, st));
+  if (pause_bytes) CK(cudaMemcpyAsync(dev + l.pause, stage + l.pause, pause_bytes, cudaMemcpyHostToDevice, st));
+  if (tail) CK(cudaMemcpyAsync(dev + l.ring, stage + l.ring, (size_t)B * kStopRing * 4, cudaMemcpyHostToDevice, st));
+  CK(cudaEventRecord(ev, st));
+  return VLY_OK;
 }
 
 // sampling == nullptr: plain greedy, no stop token (skipped when the device state already says so, unless `force`: a beam
 // search starts from that state and leaves all_done raised, so it always resets it and leaves it dirty)
+// sp with stop strings: a call that resets the flags (or sets stop_restart) uploads the tables and seeds the rings; one that
+// keeps them continues the running stop-string request.
 static int set_sampling(vly_ctx* c, vly_kv* kv, const vly_sampling* sp, bool reset_done, cudaStream_t st, bool force = false) {
   SampleState r = {};
   kv->filtered = false;
+  const bool had_stop = kv->stop_ready;
+  kv->stop_ready = false;
   if (!sp) {
     if (!kv->sample_dirty && !force) return VLY_OK;
     reset_done = true;
   } else {
+    if (sp->n_stop_strings != 0) {
+      const int V = c->cfg.vocab_size;
+      TRY(check_stop_tables(sp, kv->B, "vly_sampling"));
+      reset_done = reset_done || sp->stop_restart;
+      if (!reset_done && !had_stop)
+        return fail(VLY_ERR_STATE, "vly_generate: stop strings continue a request started by vly_sample_logits; set stop_restart to start one");
+      if (!kv->stop_buf) {
+        const StopLayout l(V);
+        TRY(kv->stop_buf.alloc(l.bytes));
+        TRY(kv->stop_stage.alloc(l.bytes, true));
+        CK(cudaEventCreateWithFlags(&kv->stop_event, cudaEventDisableTiming));
+      }
+      if (reset_done) TRY(upload_stop_tables(sp, kv->B, V, kv->stop_buf, kv->stop_stage, kv->stop_event, st));
+      stop_state(sp, kv->stop_buf, V, r);
+      kv->stop_ready = true;
+    }
     if (kv->B > kMaxSampleRows) return fail(VLY_ERR_INVALID, "sampling / eos bookkeeping supports at most %d sequences per cache", kMaxSampleRows);
     const bool on = sp->temperature >= 1e-4f;         // model_worker.py:390: below that the reference takes the arg-max
     if (on) {
@@ -1718,6 +1812,7 @@ static int set_sampling(vly_ctx* c, vly_kv* kv, const vly_sampling* sp, bool res
     r.stop2 = sp->stop_token_id < 0 ? -1 : sp->stop_token_id;
     // the filters apply only when sampling (HF ignores its warpers when it does not sample)
     kv->filtered = on && (sp->top_k > 0 || (sp->top_p > 0.f && sp->top_p < 1.f));
+    r.filter = kv->filtered ? 1 : 0;
   }
   kv->sample_dirty = sp != nullptr || force;
   return launch(c, set_sample_state_kernel, {dim3(1), dim3(64), 0, st}, kv->d_sample, r, reset_done ? 1 : 0);
@@ -1810,18 +1905,20 @@ static int generate_impl(vly_ctx* c, vly_kv* kv, const int64_t* first_tokens, in
   if (kv->host_len + n_steps > kv->Smax) return fail(VLY_ERR_INVALID, "vly_generate: %d cached + %d steps exceed the cache capacity %d", kv->host_len, n_steps, kv->Smax);
   CK(cudaSetDevice(c->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  // with a sampling struct the eos flags raised by vly_sample_logits (the first token) are kept; greedy starts clean
+  // with a sampling struct the eos flags raised by vly_sample_logits (the first token) are kept, unless a stop-string request
+  // restarts; greedy starts clean
   TRY(set_sampling(c, kv, sp, false, st));
   CK(cudaMemcpyAsync(kv->cur_tokens, first_tokens, (size_t)kv->B * 8, cudaMemcpyDeviceToDevice, st));
   CK(cudaMemsetAsync(kv->d_step, 0, 4, st));
   if (steps_done_dev) CK(cudaMemsetAsync(&kv->d_sample->steps_valid, 0, 4, st));
-  TRY(run_steps(c, kv, kv->filtered ? STEP_FILTERED : STEP_TOKEN, 0, n_steps, st));
+  // (a stop-string request selects in sample_filter_kernel, which runs the matcher)
+  TRY(run_steps(c, kv, kv->filtered || kv->stop_ready ? STEP_FILTERED : STEP_TOKEN, 0, n_steps, st));
   if (out_tokens)
     CK(cudaMemcpy2DAsync(out_tokens, (size_t)n_steps * 8, kv->gen_tokens, (size_t)kv->Smax * 8, (size_t)n_steps * 8, kv->B,
                          cudaMemcpyDeviceToDevice, st));
   if (steps_done_dev)      // (zeroed above, before the first step)
     CK(cudaMemcpyAsync(steps_done_dev, &kv->d_sample->steps_valid, 4, cudaMemcpyDeviceToDevice, st));
-  return finish_request(kv, n_steps, sp && (sp->eos_token_id >= 0 || sp->stop_token_id >= 0), st);
+  return finish_request(kv, n_steps, sp && (sp->eos_token_id >= 0 || sp->stop_token_id >= 0 || sp->n_stop_strings > 0), st);
 }
 
 extern "C" int vly_llama_decode(vly_ctx* c, vly_kv* kv, const int64_t* tokens, int64_t* next_tokens, void* logits_dev, void* stream) {
@@ -1993,10 +2090,37 @@ extern "C" int vly_test_sample_filter(vly_ctx* c, const float* logits, int B, in
   CK(cudaSetDevice(c->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   SampleState s = {};
-  s.temperature = temperature; s.inv_temp = 1.f / temperature; s.enabled = 1; s.top_k = top_k; s.top_p = top_p;
+  s.temperature = temperature; s.inv_temp = 1.f / temperature; s.enabled = 1; s.filter = 1; s.top_k = top_k; s.top_p = top_p;
   TRY(ensure(c->w_score, sizeof(SampleState)));
   CK(cudaMemcpyAsync(c->w_score.p, &s, sizeof(s), cudaMemcpyHostToDevice, st));
   return launch_sample_filter(c, logits, B, V, (SampleState*)c->w_score.p, nullptr, nullptr, nullptr, nullptr, 0, true, false, keep_out, st);
+}
+
+extern "C" int vly_test_stop_strings(vly_ctx* c, const vly_sampling* sp, int V, const int64_t* tokens, int B, int n, uint8_t* out,
+                                     void* stream) {
+  if (!c || !sp || !tokens || !out || V <= 0 || B <= 0 || B > kMaxSampleRows || n <= 0 || sp->n_stop_strings < 1)
+    return fail(VLY_ERR_INVALID, "vly_test_stop_strings: bad argument");
+  TRY(check_stop_tables(sp, B, "vly_test_stop_strings"));
+  std::lock_guard<std::mutex> lk(c->mu);
+  CK(cudaSetDevice(c->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const StopLayout l(V);
+  Owned<uint8_t> dev, stage;
+  TRY(dev.alloc(l.bytes));
+  TRY(stage.alloc(l.bytes, true));
+  cudaEvent_t ev;
+  CK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  SampleState s = {};
+  int r = upload_stop_tables(sp, 0, V, dev, stage, ev, st);
+  if (r == VLY_OK) {
+    stop_state(sp, dev, V, s);
+    r = launch(c, stop_match_test_kernel, {dim3(B), dim3(32), 0, st}, s, V, (const long long*)tokens, n, s.ring, out);
+  }
+  const cudaError_t e = cudaStreamSynchronize(st);      // (the scratch buffers are freed on return)
+  cudaEventDestroy(ev);
+  if (r != VLY_OK) return r;
+  if (e != cudaSuccess) return fail(VLY_ERR_CUDA, "vly_test_stop_strings: %s", cudaGetErrorString(e));
+  return VLY_OK;
 }
 
 // Grow-only scratch whose first `counter_bytes` are work counters: zeroed whenever the buffer is (re)allocated; the kernels

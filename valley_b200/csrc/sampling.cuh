@@ -21,17 +21,33 @@
 namespace vly {
 
 constexpr int kMaxSampleRows = 64;
+constexpr int kMaxStopStrings = 8;       // stop strings matched on the device per request
+constexpr int kMaxStopChars = 64;        // characters per device stop string: the width of the uint64 masks
+constexpr int kStopRing = 64;            // tokens of history kept per row: a match spans at most kMaxStopChars tokens
 
 struct SampleState {          // lives in device memory next to the KV cache; read by every decode step
   // the request, written by the host (set_sampling); the defaults are plain greedy with no stop token
   float temperature = 1.f;    // filtered scores are logits / temperature, an IEEE fp32 division as in HF's TemperatureLogitsWarper
   float inv_temp = 1.f;       // 1 / temperature: the draw, sample_score(logit, inv_temp, ...)
   int enabled = 0;            // 0 = greedy (scores are the raw logits: bit-identical to the plain arg-max)
+  int filter = 0;             // the request has a top-k / top-p filter (applied only by a launch that passes filter = 1)
   int top_k = 0;              // top-k filter: <= 0 off; >= V keeps every token
   float top_p = 1.f;          // top-p filter: off unless 0 < top_p < 1
   uint32_t seed_lo = 0, seed_hi = 0;
   long long eos = -1, pad = 0;  // eos < 0: no stop token
   long long stop2 = -1;       // second stop id (the worker's single-token stop string, model_worker.py:355-360); < 0: none
+  // stop strings (HF's StopStringCriteria over the tables of valley_b200/stop_strings.py); n_stop == 0: none.  A row whose
+  // text ends with one, or that emits a token of the pause set, is finished; it emits pad afterwards only when eos / stop2
+  // is set (HF pads only with an eos criterion).
+  int n_stop = 0;
+  int stop_walk = 0;          // tokens a match may span, the newest included: the longest stop string (HF's maximum_token_len)
+  int stop_len[kMaxStopStrings] = {};
+  const ulonglong2* stop_masks = nullptr;  // [n_stop][V]: x bit L-1: the token can end the string with its last L characters
+                                           //             y bit p: the token fits with its end p characters before the string's end
+  const uint8_t* tok_len = nullptr;        // [V] clean-string length of each token, capped at 255
+  const uint32_t* pause = nullptr;         // [ceil(V / 32)] bits, or null: emitting one of these tokens finishes the row
+  int* ring = nullptr;                     // [kMaxSampleRows][kStopRing]: each row's latest tokens, the next at ring_n % kStopRing
+  int ring_n[kMaxSampleRows] = {};
   // the generation's progress
   int all_done = 0;           // every row has produced eos: further steps exit at once
   int steps_valid = 0;        // decode steps executed before all_done was raised (the one that raised it included)
@@ -70,12 +86,64 @@ __device__ __forceinline__ long long sample_finish_row(SampleState* s, int b, lo
 // once every row of the step has passed sample_finish_row: count the step (count_step) and raise all_done when every row stopped
 __device__ __forceinline__ void sample_close_step(SampleState* s, int B, bool count_step) {
   if (count_step) s->steps_valid += 1;
-  if (s->eos >= 0 || s->stop2 >= 0) {
+  if (s->eos >= 0 || s->stop2 >= 0 || s->n_stop > 0) {
     const volatile int* done = s->done;             // (written by other CTAs in sample_filter_kernel)
     int all = 1;
     for (int b = 0; b < B; ++b) all &= done[b];
     s->all_done = all;
   }
+}
+
+// ---- stop strings: HF's StopStringCriteria for one row, over bit masks ----
+// The row's text is the concatenation of its tokens' clean strings (valley_b200/stop_strings.py).  With t_0 the newest token
+// and t_1, t_2, ... the ones before it, the row matches stop string i when, for some L with bit L-1 of end(i, t_0) set, the
+// walk pos = L; for j = 1, 2, ...: require bit pos of posm(i, t_j), pos += len(t_j), reaches len(i) within stop_walk tokens.
+// One warp: lane l follows the walks of L = l + 1 and l + 33.  ring: the row's latest kStopRing tokens, t_j at
+// (n - 1 - j) % kStopRing, n = tokens pushed (t_0 included).  A token id outside [0, V) fits nowhere (HF clamps it to an
+// all-empty row).  Returns the same value in every lane.
+__device__ bool stop_match_warp(const SampleState& s, int V, const int* ring, int n, long long tok, int lane) {
+  __shared__ unsigned long long pm[kStopRing];
+  __shared__ int tl[kStopRing];
+  const int walk = min(n, s.stop_walk);
+  bool loaded = false, hit = false;
+  for (int i = 0; i < s.n_stop && !hit; ++i) {
+    const ulonglong2* m = s.stop_masks + (size_t)i * V;
+    const unsigned long long end = (unsigned long long)tok < (unsigned long long)V ? m[tok].x : 0ull;
+    if (end == 0ull) continue;                     // (warp-uniform)
+    __syncwarp();
+    for (int j = 1 + lane; j < walk; j += 32) {
+      const int t = ring[(n - 1 - j) & (kStopRing - 1)];
+      const bool in = (unsigned)t < (unsigned)V;
+      pm[j] = in ? m[t].y : 0ull;
+      if (!loaded) tl[j] = in ? s.tok_len[t] : 0;
+    }
+    loaded = true;
+    __syncwarp();
+    const int len = s.stop_len[i];
+    bool mine = false;
+    for (int L = lane + 1; L <= kMaxStopChars; L += 32) {
+      if (!((end >> (L - 1)) & 1ull)) continue;
+      int pos = L;
+      for (int j = 1; pos < len && j < walk; ++j) {
+        if (!((pm[j] >> pos) & 1ull)) break;
+        pos += tl[j];
+      }
+      mine |= pos >= len;
+    }
+    hit = __any_sync(0xffffffffu, mine);
+  }
+  return hit;
+}
+
+// vly_test_stop_strings: one warp per row of tokens [B, n], read as a row whose newest token is the last: out[b] = match
+__global__ void stop_match_test_kernel(const SampleState s, int V, const long long* tokens, int n, int* ring, uint8_t* out) {
+  const int b = blockIdx.x, lane = threadIdx.x;
+  const long long* row = tokens + (size_t)b * n;
+  int* r = ring + (size_t)b * kStopRing;
+  for (int j = max(0, n - kStopRing) + lane; j < n; j += 32) r[j & (kStopRing - 1)] = (int)row[j];
+  __syncwarp();
+  const bool hit = stop_match_warp(s, V, r, n, row[n - 1], lane);
+  if (lane == 0) out[b] = hit;
 }
 
 // ---- stand-alone token selection: optional top-k / top-p (nucleus) filtering, then the Gumbel-max draw ----
@@ -93,7 +161,10 @@ __device__ __forceinline__ void sample_close_step(SampleState* s, int B, bool co
 // set and the token are a deterministic function of (logits, T, top_k, top_p, seed, row, position).
 // One CTA per row.  With a filter, the row's scores are staged in shared memory (V * 4 bytes of dynamic shared memory) when
 // they fit; otherwise every pass recomputes them from the logits in global memory.  Without one (filter = 0) the kernel draws
-// straight from the logits (the raw logit when greedy) and is launched without dynamic shared memory.
+// straight from the logits (the raw logit when greedy) and is launched without dynamic shared memory.  A launch with
+// filter = 1 filters only when the request has a filter (SampleState::filter), so stop-string requests share its graphs.
+// With stop strings, warp 0 then pushes the row's token into its ring and runs stop_match_warp (sample_filter_kernel is the
+// step's selection whenever a request has stop strings).
 constexpr int kFilterThreads = 1024;
 constexpr int kFilterStageMaxBytes = 200 * 1024;     // rows of up to 51200 scores are staged
 
@@ -128,7 +199,7 @@ __global__ void __launch_bounds__(kFilterThreads) sample_filter_kernel(const flo
   __shared__ float sh_above;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, b = blockIdx.x;
   const bool select = keep_out == nullptr;
-  if (select && per_op && !s->enabled && s->eos < 0 && s->stop2 < 0) return;   // plain greedy: the step's arg-max is the token
+  if (select && per_op && !s->enabled && s->eos < 0 && s->stop2 < 0 && s->n_stop == 0) return;   // plain greedy: the step's arg-max is the token
   if (select && s->all_done) {
     if (per_op && tid == 0) {                       // the per-op kernels keep stepping: emit pad
       next_tokens[b] = s->pad;
@@ -139,6 +210,7 @@ __global__ void __launch_bounds__(kFilterThreads) sample_filter_kernel(const flo
   const float temperature = s->temperature, top_p = s->top_p;
   const int top_k = s->top_k;
   const float* z = logits + (size_t)b * V;
+  filter = filter && (s->filter || !select);
   const bool staged = filter && (size_t)V * 4 <= (size_t)kFilterStageMaxBytes;
   auto score = [&](int n) { return staged ? srow[n] : z[n] / temperature; };
 
@@ -290,8 +362,26 @@ __global__ void __launch_bounds__(kFilterThreads) sample_filter_kernel(const flo
   bv = bv_w[lane];
   bi = bi_w[lane];
   warp_argmax(bv, bi);
-  if (lane != 0) return;
-  const long long tok = sample_finish_row(s, b, bi);
+  long long tok = bi;
+  if (s->n_stop > 0) {
+    const int was_done = s->done[b];
+    __syncwarp();
+    if (lane == 0) tok = sample_finish_row(s, b, bi);
+    tok = __shfl_sync(0xffffffffu, tok, 0);
+    if (!was_done) {
+      int* ring = s->ring + (size_t)b * kStopRing;
+      const int n = s->ring_n[b] + 1;
+      __syncwarp();
+      if (lane == 0) { ring[(n - 1) & (kStopRing - 1)] = (int)tok; s->ring_n[b] = n; }
+      bool hit = s->pause != nullptr && (unsigned long long)tok < (unsigned long long)V && ((s->pause[tok >> 5] >> (tok & 31)) & 1u);
+      if (!hit) hit = stop_match_warp(*s, V, ring, n, tok, lane);
+      if (hit && lane == 0) s->done[b] = 1;
+    }
+    if (lane != 0) return;
+  } else {
+    if (lane != 0) return;
+    tok = sample_finish_row(s, b, bi);
+  }
   next_tokens[b] = tok;
   if (out_tokens) out_tokens[(size_t)b * out_stride + (*step - 1)] = tok;
   __threadfence();

@@ -18,10 +18,12 @@ import ctypes as C
 import types
 from typing import Iterable, List, Optional, Tuple, Union
 
+import numpy as np
 import torch
 
 from . import _lib
 from . import beam as _beam
+from . import stop_strings as _ss
 from ._lib import VlyBeam, VlySampling, VlyConfig, VlyTokens, check
 
 # valley/util/config.py:1-13
@@ -329,6 +331,22 @@ class KeywordsStoppingCriteria:
 
 
 _UNSET = object()
+
+
+def host_rows_step(seq, nxt, finished, eos_token_id, pad, tables=None, stopping_criteria=None):
+    """One step of HF generate's row handling in the host-visible loop, after ``nxt`` [B] was selected for ``seq`` [B, n]:
+    finished rows emit ``pad`` when an eos criterion exists (``eos_token_id`` set); a row finishes on eos or on a stop-string
+    match (``tables``, ``stop_strings.match_rows``); the loop stops when every row has finished, or when a stopping criterion
+    returns True (a plain bool stops every row, as the reference's criteria do).  Returns (seq, nxt, finished, stop)."""
+    if eos_token_id is not None:
+        nxt = torch.where(finished, torch.full_like(nxt, pad), nxt)
+        finished = finished | (nxt == eos_token_id)
+    seq = torch.cat([seq, nxt[:, None]], dim=1)
+    if tables is not None:
+        finished = finished | _ss.match_rows(seq, tables).to(finished.device)
+    if (eos_token_id is not None or tables is not None) and bool(finished.all()):
+        return seq, nxt, finished, True
+    return seq, nxt, finished, bool(stopping_criteria) and any(sc(seq, None) for sc in stopping_criteria)
 
 
 def _repeat_rows(t: torch.Tensor, n: int) -> torch.Tensor:
@@ -722,7 +740,8 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
     @torch.no_grad()
     def generate(self, input_ids=None, images=None, max_new_tokens: int = 1024, do_sample: bool = False,
                  temperature: float = 1.0, stopping_criteria=None, eos_token_id=_UNSET, top_k=None, top_p=None,
-                 num_beams: int = 1, num_return_sequences: int = 1, length_penalty: float = 1.0, early_stopping=False, **kw):
+                 num_beams: int = 1, num_return_sequences: int = 1, length_penalty: float = 1.0, early_stopping=False,
+                 stop_strings=None, tokenizer=None, **kw):
         """Greedy (or temperature) generation == the loop of model_worker.py:371-397 / HF generate as called at
         valley_model.py:432.  Returns [B, S + n_new] like HF.  With no stopping criteria, decoding runs
         entirely on the device (CUDA-graph replay, no per-token host sync).  ``attention_mask`` [B, S] (left padding)
@@ -742,11 +761,26 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
         criteria (and up to 8 beams and 64 rows in all) the selection and the KV-cache reorder run inside the decode step's CUDA
         graph, with one device-to-host read per request; otherwise a host-visible loop runs the same search
         (valley_b200/beam.py).  The returned sequences' scores (HF's ``sequences_scores``) are left in
-        ``model.last_beam_scores``.  Beam sampling (``do_sample=True``) is not implemented."""
+        ``model.last_beam_scores``.  Beam sampling (``do_sample=True``) is not implemented.
+
+        ``stop_strings`` (a string or a list of strings) with ``tokenizer``: transformers' ``StopStringCriteria``.  A row
+        finishes when its text ends with a stop string, the last characters inside the newest token; the text is the
+        concatenation of the tokens' clean strings (``valley_b200/stop_strings.py``), prompt included.  Finished rows are padded
+        only when ``eos_token_id`` is set, as in HF; generation ends when every row has finished.  With ``num_beams == 1``, no
+        other stopping criteria, at most 64 rows, at most 8 stop strings and at most 64 characters each, the matcher runs on
+        the device after every token (no per-token host sync); otherwise the host-visible loops check it.  ``stop_strings``
+        without ``tokenizer`` raises HF's ``ValueError``."""
         B, S = input_ids.shape
+        tables = None
+        if stop_strings is not None:
+            if tokenizer is None:
+                raise ValueError("There are one or more stop strings, either in the arguments to `generate` or in the model's "
+                                 "generation config, but we could not locate a tokenizer. When generating with stop strings, "
+                                 "you must pass the model's tokenizer to the `tokenizer` argument of `generate`.")
+            tables = _ss.stop_tables(_ss.clean_token_strings(tokenizer), stop_strings, self.config.vocab_size)
         if num_beams != 1:
             return self._beam_generate(input_ids, images, max_new_tokens, do_sample, stopping_criteria, eos_token_id, num_beams,
-                                       num_return_sequences, length_penalty, early_stopping, **kw)
+                                       num_return_sequences, length_penalty, early_stopping, tables=tables, **kw)
         greedy = (not do_sample) or temperature < 1e-4
         filters = {} if greedy else dict(zip(("top_k", "top_p"), sampling_filters(top_k, top_p)))
         n_new, eos_token_id, pad_token_id, attention_mask = self._generation_defaults(input_ids, max_new_tokens, eos_token_id, kw)
@@ -757,7 +791,7 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
         try:
             cache.set_attention_mask(attention_mask, S)
             return self._generate_with_cache(cache, input_ids, embeds, n_new, do_sample, temperature, stopping_criteria, eos_token_id,
-                                             pad_token_id, **filters)
+                                             pad_token_id, tables=tables, **filters)
         finally:
             cache.release()
 
@@ -779,13 +813,17 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
         return n_new, eos_token_id, pad_token_id, attention_mask
 
     def _generate_with_cache(self, cache, input_ids, embeds, n_new, do_sample, temperature, stopping_criteria, eos_token_id,
-                             pad_token_id=None, top_k=0, top_p=1.0):
+                             pad_token_id=None, top_k=0, top_p=1.0, tables=None):
         B = input_ids.shape[0]
         greedy = (not do_sample) or temperature < 1e-4
-        device_select = not stopping_criteria and not (greedy and eos_token_id is None) and B <= 64
+        device_select = (not stopping_criteria and not (greedy and eos_token_id is None and tables is None) and B <= 64
+                         and (tables is None or tables.on_device))
+        tail = None
+        if device_select and tables is not None:       # the prompt's last tokens seed the device matcher (the whole row counts)
+            tail = input_ids[:, -min(input_ids.shape[1], 63):].to("cpu", torch.int64).numpy()
         logits, nxt = self._prefill(cache, embeds, 0 if (greedy and not device_select) else 1)
         ids_dev = input_ids.to(self.device, torch.int64)
-        if greedy and not stopping_criteria and eos_token_id is None:
+        if greedy and not stopping_criteria and eos_token_id is None and tables is None:
             out = torch.empty(B, n_new, dtype=torch.int64, device=self.device)
             out[:, 0] = nxt
             if n_new > 1:
@@ -801,6 +839,8 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())                         # torch.manual_seed() governs it
             # (a top-k / top-p filter: one more kernel per step selects over the step's logits, still on the device)
             sp = VlySampling(0.0 if greedy else float(temperature), seed, eos, pad, top_k=top_k, top_p=top_p)
+            if tables is not None:
+                sp.set_stop_strings(tables, tail)
             out = torch.empty(B, n_new, dtype=torch.int64, device=self.device)
             first = torch.empty(B, dtype=torch.int64, device=self.device)
             check(self._lib.vly_sample_logits(self._ctx, cache._h, logits.data_ptr(), C.byref(sp), first.data_ptr(), _stream()))
@@ -814,8 +854,8 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
                 out[:, 1:] = rest
                 n_valid += int(done.item())
             return torch.cat([ids_dev, out[:, :n_valid]], dim=1)
-        # host-visible loop (stopping criteria present, or B > 64): one device->host sync per token, as in the reference.
-        # HF semantics per row: a row that has emitted eos is finished and is fed / emits pad from then on
+        # host-visible loop (stopping criteria present, B > 64, or stop strings past the device limits): one device->host
+        # sync per token, as in the reference
         seq = ids_dev
         finished = torch.zeros(B, dtype=torch.bool, device=self.device)
         pad = int(pad_token_id) if pad_token_id is not None else (int(eos_token_id) if eos_token_id is not None else 0)
@@ -824,20 +864,15 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
                 scores = filter_scores(logits[:, -1, :] / temperature, top_k, top_p)     # model_worker.py:393-394
                 probs = torch.softmax(scores, dim=-1)
                 nxt = torch.multinomial(probs, num_samples=1).reshape(B)
-            if eos_token_id is not None:
-                nxt = torch.where(finished, torch.full_like(nxt, pad), nxt)
-                finished = finished | (nxt == eos_token_id)
-            seq = torch.cat([seq, nxt[:, None]], dim=1)
-            if eos_token_id is not None and bool(finished.all()):
-                break
-            if stopping_criteria and any(sc(seq, None) for sc in stopping_criteria):
+            seq, nxt, finished, stop = host_rows_step(seq, nxt, finished, eos_token_id, pad, tables, stopping_criteria)
+            if stop:
                 break
             if i + 1 < n_new:
                 logits, nxt = self._decode(cache, nxt, not greedy)
         return seq
 
     def _beam_generate(self, input_ids, images, max_new_tokens, do_sample, stopping_criteria, eos_token_id, num_beams,
-                       num_return_sequences, length_penalty, early_stopping, **kw):
+                       num_return_sequences, length_penalty, early_stopping, tables=None, **kw):
         """generate(num_beams > 1): the vision part is encoded once per row, then every row's embeddings and attention mask
         are repeated num_beams times (HF's _expand_inputs_for_generation) and prefilled as B * num_beams cache rows."""
         if not isinstance(num_beams, int) or num_beams < 1:
@@ -865,7 +900,7 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
             cache.set_attention_mask(attention_mask, S)
             logits, _ = self._prefill(cache, embeds, 1)
             logits = logits[:, -1].contiguous()
-            if not stopping_criteria and nb <= 8 and B * nb <= 64:
+            if not stopping_criteria and tables is None and nb <= 8 and B * nb <= 64:
                 nrs = num_return_sequences
                 es = {False: 0, True: 1, "never": 2}[early_stopping]
                 bp = VlyBeam(nb, nrs, float(length_penalty), es, -1 if eos_token_id is None else int(eos_token_id), fill)
@@ -881,11 +916,13 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
             # candidates (a criterion returning a plain bool applies to every row, as in HF's StoppingCriteriaList)
             bs = _beam.BeamSearch(ids_rep, nb, n_new, eos_token_id, fill, length_penalty, early_stopping)
             stop = None
-            if stopping_criteria:
+            if stopping_criteria or tables is not None:
                 def stop(seqs):
                     done = torch.zeros(seqs.shape[0], dtype=torch.bool, device=seqs.device)
-                    for sc in stopping_criteria:
+                    for sc in stopping_criteria or ():
                         done = done | torch.as_tensor(sc(seqs, None), device=seqs.device)
+                    if tables is not None:
+                        done = done | _ss.match_rows(seqs, tables).to(seqs.device)
                     return done
             while True:
                 parents, tokens = bs.step(logits, stop)
@@ -896,6 +933,74 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
                 logits = step_logits[:, -1]
             out, self.last_beam_scores = bs.result(num_return_sequences)
             return out
+        finally:
+            cache.release()
+
+    _KEYWORD_ROUTE_ARGS = frozenset({"max_new_tokens", "do_sample", "temperature", "eos_token_id", "pad_token_id",
+                                     "attention_mask", "top_k", "top_p", "num_beams", "use_cache"})
+
+    def _keyword_generate(self, input_ids, images, criterion: KeywordsStoppingCriteria, gen_kwargs):
+        """``generate(stopping_criteria=[criterion], **gen_kwargs)`` for a greedy single-row request, with the keyword matched
+        on the device instead of decoding the reply after every token; None when the request does not qualify (sampled,
+        beams, more rows, other arguments, or a keyword past the device limits), and the host loop runs it instead.
+
+        The criterion decides, as in the host loop: it is called after the first token (which only records the prompt
+        length), and again whenever the device loop stops early -- on a stop-string match of a keyword over the generated
+        tokens, or on a token the criterion's decode deletes (``stop_strings.pause_bits``: such a token can join two halves
+        of a keyword) -- and True ends the request, False resumes the device loop.  A first token whose own text holds a
+        keyword is followed by one host step, as the host loop's criterion only sees it then."""
+        kw = dict(gen_kwargs)
+        greedy = not kw.pop("do_sample", False) or kw.pop("temperature", 1.0) < 1e-4
+        kw.pop("temperature", None)
+        if (not greedy or kw.pop("num_beams", 1) != 1 or input_ids.shape[0] != 1 or set(kw) - self._KEYWORD_ROUTE_ARGS
+                or not hasattr(criterion.tokenizer, "get_vocab")):
+            return None
+        tok = criterion.tokenizer
+        V = self.config.vocab_size
+        tables = _ss.stop_tables(_ss.clean_token_strings(tok), criterion.keywords, V)
+        if not tables.on_device:
+            return None
+        S = input_ids.shape[1]
+        n_new, eos, pad, attention_mask = self._generation_defaults(input_ids, kw.get("max_new_tokens", 1024),
+                                                                    kw.get("eos_token_id", _UNSET), kw)
+        if n_new == 0:
+            return None
+        pause = _ss.pause_bits(tok, V, exclude=() if eos is None else (int(eos),))
+        paused = lambda t: bool((int(pause[t >> 5]) >> (t & 31)) & 1) if 0 <= t < V else False
+        _, _, _, embeds, _ = self.prepare_inputs_labels_for_multimodal(input_ids, None, None, None, images)
+        cache = self.new_cache(1)
+        try:
+            cache.set_attention_mask(attention_mask, S)
+            _, nxt = self._prefill(cache, embeds, 0)
+            seq = torch.cat([input_ids.to(self.device, torch.int64), nxt[:, None]], dim=1)
+            gen = [int(nxt.item())]
+            if eos is not None and gen[0] == eos:
+                return seq
+            if criterion(seq, None):                        # (records the prompt length)
+                return seq
+            if len(gen) < n_new and any(k in tok.decode(gen[:1], skip_special_tokens=True) for k in criterion.keywords):
+                _, nxt = self._decode(cache, nxt, False)
+                seq = torch.cat([seq, nxt[:, None]], dim=1)
+                gen.append(int(nxt.item()))
+                if (eos is not None and gen[-1] == eos) or criterion(seq, None):
+                    return seq
+            last = nxt
+            while len(gen) < n_new:
+                n = n_new - len(gen)
+                tail = [t for t in gen if not paused(t)][-63:]
+                sp = VlySampling(0.0, 0, -1 if eos is None else int(eos), int(pad) if pad is not None else 0)
+                sp.set_stop_strings(tables, np.asarray([tail], dtype=np.int64).reshape(1, len(tail)), pause, restart=True)
+                rest = torch.empty(1, n, dtype=torch.int64, device=self.device)
+                done = torch.zeros(1, dtype=torch.int32, device=self.device)
+                check(self._lib.vly_generate(self._ctx, cache._h, last.reshape(1).contiguous().data_ptr(), n, rest.data_ptr(),
+                                             C.byref(sp), done.data_ptr(), _stream()))
+                k = int(done.item())
+                seq = torch.cat([seq, rest[:, :k]], dim=1)
+                gen += rest[0, :k].tolist()
+                if k == n or (eos is not None and gen[-1] == eos) or criterion(seq, None):
+                    break
+                last = rest[:, k - 1].clone()
+            return seq
         finally:
             cache.release()
 
@@ -965,7 +1070,9 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
                 and getattr(self.config, "eos_token_id", None) is None:
             gen_kwargs["eos_token_id"] = tokenizer.eos_token_id
         stopping_criteria = KeywordsStoppingCriteria(['###'], tokenizer, input_ids)
-        output_ids = self.generate(input_ids=input_ids, images=images, stopping_criteria=[stopping_criteria], **gen_kwargs)
+        output_ids = self._keyword_generate(input_ids, images, stopping_criteria, gen_kwargs)
+        if output_ids is None:
+            output_ids = self.generate(input_ids=input_ids, images=images, stopping_criteria=[stopping_criteria], **gen_kwargs)
         input_token_len = input_ids.shape[1]
         n_diff_input_output = (input_ids != output_ids[:, :input_token_len]).sum().item()
         if n_diff_input_output > 0:
