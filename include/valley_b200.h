@@ -225,6 +225,14 @@ typedef struct {
   int32_t stop_restart;            /* vly_generate: 1 = start the matcher here (upload the tables, seed the rows from stop_tail
                                     * and clear the finished flags); 0 = continue the request vly_sample_logits started.
                                     * vly_sample_logits always starts it. */
+  /* Recording (HF generate's output_scores / output_logits): device buffers [n_slots, B, V] fp32 owned by the caller, or NULL.
+   * vly_sample_logits writes slot 0; vly_generate writes slot i for its step i (pass pointers offset by one slot to continue
+   * the request vly_sample_logits started).  scores_out: the scores the token is selected from -- logits / temperature when
+   * temperature > 0 (the raw logits when it is 0), with -inf at every token the top-k / top-p filter removed; logits_out:
+   * the raw logits.  Every row is recorded, finished ones too; nothing is recorded after every row has finished.  A request
+   * that records selects in the filtered-token step (one more kernel per step at B <= 4).  NULL: nothing is recorded. */
+  float* scores_out;
+  float* logits_out;
 } vly_sampling;
 
 /* the first generated token: select from the prefill's last-position logits [B,V] fp32 (vly_llama_prefill logits_mode 1);
@@ -252,6 +260,18 @@ typedef struct {
   int32_t early_stopping;        /* 0: False (HF default), 1: True, 2: "never"                                  */
   int64_t eos_token_id;          /* -1: none                                                                    */
   int64_t pad_token_id;          /* written beyond each sequence's end (HF's output_fill_value)                  */
+  /* Recording (HF's output_scores / output_logits / beam_indices), device buffers owned by the caller, or NULL:
+   *   scores_out / logits_out [n_steps, B, V] fp32: slot t = search step t (the first one selects from first_logits_dev):
+   *     HF's log_probs (log_softmax of every beam row, float64 log-sum-exp, before the beam scores are added) / the raw logits;
+   *   beam_indices_out [B / num_beams * num_return_sequences, n_steps] int64: per returned hypothesis and step, the cache row
+   *     (item * num_beams + beam) the token was appended to, -1 from the hypothesis' generated length on;
+   *   steps_out (one int32): the search steps run (HF's len(scores)).
+   * The library allocates nothing per request for these; the beam-index rows it keeps on the device are allocated with the
+   * cache's other beam buffers, on its first beam request. */
+  float* scores_out;
+  float* logits_out;
+  int64_t* beam_indices_out;
+  int32_t* steps_out;
 } vly_beam;
 
 /* Beam search after the prefill of the prompt_len-token prompt (the cache's length): the first step selects from

@@ -38,7 +38,8 @@ class VlySampling(C.Structure):
                 ("stop_token_id", C.c_int64), ("top_k", C.c_int32), ("top_p", C.c_float),
                 ("n_stop_strings", C.c_int32), ("stop_lens", C.POINTER(C.c_int32)), ("stop_masks", C.POINTER(C.c_uint64)),
                 ("stop_token_lens", C.POINTER(C.c_int32)), ("pause_bits", C.POINTER(C.c_uint32)),
-                ("stop_tail", C.POINTER(C.c_int64)), ("stop_tail_len", C.c_int32), ("stop_restart", C.c_int32)]
+                ("stop_tail", C.POINTER(C.c_int64)), ("stop_tail_len", C.c_int32), ("stop_restart", C.c_int32),
+                ("scores_out", C.c_void_p), ("logits_out", C.c_void_p)]
 
     def __init__(self, temperature=0.0, seed=0, eos_token_id=-1, pad_token_id=0, stop_token_id=-1, top_k=0, top_p=1.0):
         super().__init__(temperature, seed, eos_token_id, pad_token_id, stop_token_id, top_k, top_p)
@@ -73,7 +74,9 @@ class VlySampling(C.Structure):
 
 class VlyBeam(C.Structure):
     _fields_ = [("num_beams", C.c_int32), ("num_return_sequences", C.c_int32), ("length_penalty", C.c_float),
-                ("early_stopping", C.c_int32), ("eos_token_id", C.c_int64), ("pad_token_id", C.c_int64)]
+                ("early_stopping", C.c_int32), ("eos_token_id", C.c_int64), ("pad_token_id", C.c_int64),
+                ("scores_out", C.c_void_p), ("logits_out", C.c_void_p), ("beam_indices_out", C.c_void_p),
+                ("steps_out", C.c_void_p)]
 
 
 VLY_OK, VLY_ERR_INVALID, VLY_ERR_CUDA, VLY_ERR_STATE = 0, -1, -2, -3

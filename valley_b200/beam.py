@@ -43,10 +43,13 @@ class BeamSearch:
 
     ``step(logits)`` takes the step's logits [B * num_beams, V] and returns ``(parent_rows, tokens)``: the row of the previous
     step every new beam continues (what the KV cache must be reordered by) and the tokens to feed next; ``done`` is set when
-    HF's loop would stop.  ``result(num_return_sequences)`` gives ``(sequences [B * nrs, S + L], sequences_scores [B * nrs])``."""
+    HF's loop would stop.  ``result(num_return_sequences)`` gives ``(sequences [B * nrs, S + L], sequences_scores [B * nrs])``,
+    ``beam_indices(num_return_sequences)`` HF's ``beam_indices`` [B * nrs, L] next to them.  ``record_scores`` / ``record_logits``
+    keep every step's log-probabilities / logits [B * num_beams, V] in ``scores`` / ``logits`` (HF's output_scores /
+    output_logits); ``t`` is the number of steps run."""
 
     def __init__(self, prompt_ids: torch.Tensor, num_beams: int, max_new_tokens: int, eos_token_id: Optional[int], fill: int,
-                 length_penalty: float = 1.0, early_stopping=False):
+                 length_penalty: float = 1.0, early_stopping=False, record_scores: bool = False, record_logits: bool = False):
         rows, S = prompt_ids.shape
         self.nb, self.B, self.S, self.n_new = num_beams, rows // num_beams, S, max_new_tokens
         self.K = 2 * num_beams                     # max(2, 1 + n_eos) * num_beams with at most one eos id
@@ -62,6 +65,11 @@ class BeamSearch:
         self.fin_len = torch.zeros(self.B, num_beams, dtype=torch.int64, device=dev)
         self.heur = torch.ones(self.B, 1, dtype=torch.bool, device=dev)
         self.top_mask = (torch.arange(self.K, device=dev) < num_beams)[None]
+        # beam indices of the running / finished hypotheses: per generated position, the cache row the token was appended to
+        self.bidx = torch.full((self.B, num_beams, max_new_tokens), -1, dtype=torch.int64, device=dev)
+        self.fin_bidx = self.bidx.clone()
+        self.scores = [] if record_scores else None
+        self.logits = [] if record_logits else None
         self.t, self.done = 0, False
         self.margins = []                          # per step: the smallest gap between consecutive top-(K+1) candidates
 
@@ -72,13 +80,20 @@ class BeamSearch:
         B, nb, K, t = self.B, self.nb, self.K, self.t
         V = logits.shape[-1]
         cur = self.S + t
-        acc = (log_softmax(logits.float()).reshape(B, nb, V) + self.run_scores[:, :, None]).reshape(B, nb * V)
+        log_probs = log_softmax(logits.float())
+        if self.scores is not None:
+            self.scores.append(log_probs)
+        if self.logits is not None:
+            self.logits.append(logits.float())
+        acc = (log_probs.reshape(B, nb, V) + self.run_scores[:, :, None]).reshape(B, nb * V)
         top_v, top_i = topk(acc, K + 1)
         self.margins.append(float((top_v[:, :-1] - top_v[:, 1:]).min()))
         vals, idx = top_v[:, :K], top_i[:, :K]
         parent, tok = idx // V, idx % V
         cand = torch.take_along_dim(self.seq, parent[:, :, None], dim=1)
         cand[:, :, cur] = tok
+        cand_bidx = torch.take_along_dim(self.bidx, parent[:, :, None], dim=1)
+        cand_bidx[:, :, t] = parent + torch.arange(B, device=parent.device)[:, None] * nb
         hits = tok == self.eos if self.eos is not None else torch.zeros_like(tok, dtype=torch.bool)
         if t + 1 >= self.n_new:                    # MaxLengthCriteria
             hits = torch.ones_like(hits)
@@ -89,6 +104,7 @@ class BeamSearch:
         adj = vals + hits.to(torch.float32) * NEG
         run_v, run_i = topk(adj, nb)
         self.seq = torch.take_along_dim(cand, run_i[:, :, None], dim=1)
+        self.bidx = torch.take_along_dim(cand_bidx, run_i[:, :, None], dim=1)
         self.run_scores = run_v
         run_parent = torch.take_along_dim(parent, run_i, dim=1)
         # the finished hypotheses (_update_finished_beams)
@@ -103,6 +119,7 @@ class BeamSearch:
         m_len = torch.cat((self.fin_len, torch.full_like(vals, t + 1, dtype=torch.int64)), 1)
         _, mi = topk(m_s, nb)
         self.fin_seq = torch.take_along_dim(m_seq, mi[:, :, None], dim=1)
+        self.fin_bidx = torch.take_along_dim(torch.cat((self.fin_bidx, cand_bidx), 1), mi[:, :, None], dim=1)
         self.fin_scores = torch.take_along_dim(m_s, mi, dim=1)
         self.fin = torch.take_along_dim(m_f, mi, dim=1)
         self.fin_len = torch.take_along_dim(m_len, mi, dim=1)
@@ -121,3 +138,9 @@ class BeamSearch:
         seq = self.fin_seq[:, :n].reshape(self.B * n, -1)
         L = int(self.fin_len[:, :n].max())
         return seq[:, :self.S + L], self.fin_scores[:, :n].reshape(-1)
+
+    def beam_indices(self, num_return_sequences: int = 1) -> torch.Tensor:
+        """HF's ``beam_indices`` of the hypotheses ``result`` returns: [B * nrs, L] int64, -1 after each one's end"""
+        n = num_return_sequences
+        L = int(self.fin_len[:, :n].max())
+        return self.fin_bidx[:, :n].reshape(self.B * n, -1)[:, :L]

@@ -233,13 +233,16 @@ struct vly_kv {
   Owned<SampleState> d_sample;        // token selection state read by every decode step (sampling.cuh)
   bool sample_dirty = false;          // device state is not the plain-greedy default
   bool filtered = false;              // the last sampling set has a top-k / top-p filter: sample_filter_kernel selects
+  bool recording = false;             // the last sampling set records scores or logits: sample_filter_kernel selects
   Owned<uint32_t> key_bits;           // [B, Smax/32] attention_mask bits (1 = attend); all ones unless vly_kv_set_key_mask
   bool masked = false;
   int mask_words() const { return Smax / 32; }
   // beam search (vly_beam_search), allocated on the cache's first beam request: the state, the running and finished token
-  // rows [2 parities][2][B][Smax] and the length-penalty divisors [Smax]
+  // rows [2 parities][2][B][Smax], their beam-index rows (same layout, int32; written only by requests that record beam
+  // indices) and the length-penalty divisors [Smax]
   Owned<BeamState> d_beam;
   Owned<long long> beam_tok;
+  Owned<int> beam_bidx;
   Owned<float> beam_div;
   Owned<int> beam_from;               // vly_kv_beam_reorder's first position
   // stop strings (set_sampling), allocated on the cache's first stop-string request: the tables and the per-row token rings
@@ -1670,9 +1673,10 @@ static int launch_kv_beam_reorder(vly_ctx* c, vly_kv* kv, int group, const int* 
 }
 
 static int launch_beam_step(vly_ctx* c, vly_kv* kv, int nb, const float* logits, cudaStream_t st) {
-  long long* fin = kv->beam_tok + (size_t)2 * kv->B * kv->Smax;
+  const size_t half = (size_t)2 * kv->B * kv->Smax;       // [2 parities][B][Smax]: the running rows, then the finished ones
   return launch(c, beam_step_kernel, {dim3(kv->B / nb), dim3(kBeamThreads), 0, st}, logits, c->cfg.vocab_size, kv->d_beam,
-                (long long*)kv->beam_tok, fin, kv->Smax, (const float*)kv->beam_div, (long long*)kv->cur_tokens, kv->d_sample);
+                (long long*)kv->beam_tok, kv->beam_tok + half, (int*)kv->beam_bidx, kv->beam_bidx + half, kv->Smax,
+                (const float*)kv->beam_div, (long long*)kv->cur_tokens, kv->d_sample);
 }
 
 // Enqueue one decode step of kv: the persistent kernel (B <= 4) or the per-op kernels per group of <= 4 rows, then what the
@@ -1700,7 +1704,7 @@ __global__ void set_sample_state_kernel(SampleState* s, const SampleState r, int
     s->temperature = r.temperature; s->inv_temp = r.inv_temp; s->enabled = r.enabled; s->filter = r.filter; s->top_k = r.top_k;
     s->top_p = r.top_p; s->seed_lo = r.seed_lo; s->seed_hi = r.seed_hi; s->eos = r.eos; s->pad = r.pad; s->stop2 = r.stop2;
     s->n_stop = r.n_stop; s->stop_walk = r.stop_walk; s->stop_masks = r.stop_masks; s->tok_len = r.tok_len; s->pause = r.pause;
-    s->ring = r.ring;
+    s->ring = r.ring; s->rec_scores = r.rec_scores; s->rec_logits = r.rec_logits; s->rec_temp = r.rec_temp;
     if (reset_done) { s->all_done = 0; s->steps_valid = 0; }
   }
   if (threadIdx.x < kMaxStopStrings) s->stop_len[threadIdx.x] = r.stop_len[threadIdx.x];
@@ -1779,6 +1783,7 @@ static int upload_stop_tables(const vly_sampling* sp, int B, int V, uint8_t* dev
 static int set_sampling(vly_ctx* c, vly_kv* kv, const vly_sampling* sp, bool reset_done, cudaStream_t st, bool force = false) {
   SampleState r = {};
   kv->filtered = false;
+  kv->recording = false;
   const bool had_stop = kv->stop_ready;
   kv->stop_ready = false;
   if (!sp) {
@@ -1813,6 +1818,11 @@ static int set_sampling(vly_ctx* c, vly_kv* kv, const vly_sampling* sp, bool res
     // the filters apply only when sampling (HF ignores its warpers when it does not sample)
     kv->filtered = on && (sp->top_k > 0 || (sp->top_p > 0.f && sp->top_p < 1.f));
     r.filter = kv->filtered ? 1 : 0;
+    // recording: HF records logits / temperature whenever it samples, also where the temperature is too low to draw with
+    r.rec_scores = sp->scores_out;
+    r.rec_logits = sp->logits_out;
+    r.rec_temp = sp->temperature > 0.f ? sp->temperature : 1.f;
+    kv->recording = sp->scores_out != nullptr || sp->logits_out != nullptr;
   }
   kv->sample_dirty = sp != nullptr || force;
   return launch(c, set_sample_state_kernel, {dim3(1), dim3(64), 0, st}, kv->d_sample, r, reset_done ? 1 : 0);
@@ -1881,7 +1891,8 @@ extern "C" int vly_sample_logits(vly_ctx* c, vly_kv* kv, const float* logits, co
   CK(cudaSetDevice(c->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
   TRY(set_sampling(c, kv, sp, true, st));
-  return launch_sample_filter(c, logits, kv->B, c->cfg.vocab_size, kv->d_sample, kv->d_len, kv->d_step, (long long*)tokens_out, nullptr,
+  // (no step counter: the first token records into slot 0)
+  return launch_sample_filter(c, logits, kv->B, c->cfg.vocab_size, kv->d_sample, kv->d_len, nullptr, (long long*)tokens_out, nullptr,
                               0, kv->filtered, false, nullptr, st);
 }
 
@@ -1911,8 +1922,8 @@ static int generate_impl(vly_ctx* c, vly_kv* kv, const int64_t* first_tokens, in
   CK(cudaMemcpyAsync(kv->cur_tokens, first_tokens, (size_t)kv->B * 8, cudaMemcpyDeviceToDevice, st));
   CK(cudaMemsetAsync(kv->d_step, 0, 4, st));
   if (steps_done_dev) CK(cudaMemsetAsync(&kv->d_sample->steps_valid, 0, 4, st));
-  // (a stop-string request selects in sample_filter_kernel, which runs the matcher)
-  TRY(run_steps(c, kv, kv->filtered || kv->stop_ready ? STEP_FILTERED : STEP_TOKEN, 0, n_steps, st));
+  // (a stop-string request selects in sample_filter_kernel, which runs the matcher; a recording one, which writes its slot)
+  TRY(run_steps(c, kv, kv->filtered || kv->stop_ready || kv->recording ? STEP_FILTERED : STEP_TOKEN, 0, n_steps, st));
   if (out_tokens)
     CK(cudaMemcpy2DAsync(out_tokens, (size_t)n_steps * 8, kv->gen_tokens, (size_t)kv->Smax * 8, (size_t)n_steps * 8, kv->B,
                          cudaMemcpyDeviceToDevice, st));
@@ -1944,6 +1955,7 @@ static int ensure_beam_buffers(vly_kv* kv) {
   if (kv->d_beam) return VLY_OK;
   TRY(kv->d_beam.alloc(sizeof(BeamState)));
   TRY(kv->beam_tok.alloc((size_t)4 * kv->B * kv->Smax * sizeof(long long)));
+  TRY(kv->beam_bidx.alloc((size_t)4 * kv->B * kv->Smax * sizeof(int)));
   TRY(kv->beam_div.alloc((size_t)kv->Smax * sizeof(float)));
   TRY(kv->beam_from.alloc(sizeof(int)));
   return VLY_OK;
@@ -1969,13 +1981,15 @@ extern "C" int vly_beam_search(vly_ctx* c, vly_kv* kv, const vly_beam* bp, const
   // plain selection state: the decode steps write logits only, and exit once beam_step_kernel raises all_done
   TRY(set_sampling(c, kv, nullptr, true, st, true));
   TRY(launch(c, beam_init_kernel, {dim3(1), dim3(256), 0, st}, kv->d_beam, kv->B, nb, n_steps, prompt_len, (int)bp->early_stopping,
-             bp->length_penalty, (long long)(bp->eos_token_id < 0 ? -1 : bp->eos_token_id), (float*)kv->beam_div));
+             bp->length_penalty, (long long)(bp->eos_token_id < 0 ? -1 : bp->eos_token_id), (float*)kv->beam_div, bp->scores_out,
+             bp->logits_out, (long long*)bp->beam_indices_out, (int*)bp->steps_out));
   TRY(launch_beam_step(c, kv, nb, first_logits, st));
   CK(cudaMemsetAsync(kv->d_step, 0, 4, st));
   TRY(run_steps(c, kv, STEP_BEAM, nb, n_steps - 1, st));
-  const long long* fin = kv->beam_tok + (size_t)2 * kv->B * kv->Smax;
-  TRY(launch(c, beam_output_kernel, {dim3(kv->B / nb * nrs), dim3(256), 0, st}, (const BeamState*)kv->d_beam, fin, kv->Smax, kv->B, nrs,
-             n_steps, (long long)bp->pad_token_id, (long long*)seq_out, scores_out, gen_len_out));
+  const size_t half = (size_t)2 * kv->B * kv->Smax;
+  TRY(launch(c, beam_output_kernel, {dim3(kv->B / nb * nrs), dim3(256), 0, st}, (const BeamState*)kv->d_beam,
+             (const long long*)kv->beam_tok + half, (const int*)kv->beam_bidx + half, kv->Smax, kv->B, nrs, n_steps,
+             (long long)bp->pad_token_id, (long long*)seq_out, scores_out, gen_len_out));
   // the steps after the end of the search did not advance the cache
   return finish_request(kv, n_steps - 1, true, st);
 }

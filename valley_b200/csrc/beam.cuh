@@ -44,15 +44,23 @@ struct BeamState {            // device memory, one per KV cache that ran a beam
   int fin_flag[kMaxSampleRows];      // per row: is_sent_finished
   int fin_len[kMaxSampleRows];       // per row: generated length of the finished hypothesis
   int parent[kMaxSampleRows];        // per row: the cache row the running beam continues (the reorder's source)
+  // recording (vly_beam's output pointers, caller buffers, or null): slot `step` of rec_scores / rec_logits [n_steps][rows][V]
+  // gets each beam row's log-probabilities / raw logits; with bidx_out the step also keeps the beam-index rows
+  float* rec_scores;
+  float* rec_logits;
+  long long* bidx_out;
+  int* steps_out;
 };
 
 // Starts a request: rows = items * nb.  lp_div[L - 1] = (float)pow(L, length_penalty), L = 1 .. n_steps (Python's int ** float).
 __global__ void beam_init_kernel(BeamState* s, int rows, int nb, int n_steps, int prompt_len, int early_stopping,
-                                 float length_penalty, long long eos, float* lp_div) {
+                                 float length_penalty, long long eos, float* lp_div, float* rec_scores, float* rec_logits,
+                                 long long* bidx_out, int* steps_out) {
   const int tid = threadIdx.x;
   if (tid == 0) {
     s->nb = nb; s->K = 2 * nb; s->n_steps = n_steps; s->prompt_len = prompt_len; s->early_stopping = early_stopping;
     s->lp_positive = length_penalty > 0.f; s->eos = eos; s->step = 0; s->done = 0; s->arrive = 0;
+    s->rec_scores = rec_scores; s->rec_logits = rec_logits; s->bidx_out = bidx_out; s->steps_out = steps_out;
   }
   for (int r = tid; r < kMaxSampleRows; r += blockDim.x) {
     s->heur[r] = 1; s->open[r] = 1;
@@ -67,11 +75,12 @@ __device__ __forceinline__ bool beam_better(float av, int ai, float bv, int bi) 
 
 // One beam-search step for item blockIdx.x (rows [g * nb, g * nb + nb)): reads the step's logits [rows, V], selects, writes the
 // running and finished token rows of the next step (double-buffered by the parity of the step: buffer p of run_tok / fin_tok is
-// [rows][stride]), the next input tokens and the parent rows.  The last CTA to finish decides whether the search goes on and
+// [rows][stride]), the next input tokens and the parent rows.  A request that records beam indices keeps a beam-index row
+// next to every token row the same way (run_bi / fin_bi, int32: entry p is the cache row the token at p was appended to).  The last CTA to finish decides whether the search goes on and
 // raises SampleState::all_done when it ends, so that the remaining decode steps exit at once.
 __global__ void __launch_bounds__(kBeamThreads) beam_step_kernel(const float* __restrict__ logits, int V, BeamState* s,
-                                                                 long long* run_tok, long long* fin_tok, int stride,
-                                                                 const float* __restrict__ lp_div, long long* cur_tokens,
+                                                                 long long* run_tok, long long* fin_tok, int* run_bi, int* fin_bi,
+                                                                 int stride, const float* __restrict__ lp_div, long long* cur_tokens,
                                                                  SampleState* ss) {
   __shared__ float red_f[32];
   __shared__ double red_d[32];
@@ -120,8 +129,14 @@ __global__ void __launch_bounds__(kBeamThreads) beam_step_kernel(const float* __
     const float* z = logits + (size_t)(r0 + j) * V;
     const double l = lse[j];
     const float rs = s->run_score[r0 + j];
+    const size_t rec = ((size_t)t * rows + r0 + j) * V;         // the row's slot in the recorded [step][row][V] buffers
+    float* rec_s = s->rec_scores ? s->rec_scores + rec : nullptr;
+    float* rec_l = s->rec_logits ? s->rec_logits + rec : nullptr;
     for (int n = tid; n < V; n += kBeamThreads) {
-      float v = (float)((double)z[n] - l) + rs;
+      const float lp = (float)((double)z[n] - l);
+      if (rec_s) rec_s[n] = lp;
+      if (rec_l) rec_l[n] = z[n];
+      float v = lp + rs;
       int i = j * V + n;
       if (!beam_better(v, i, lv[kBeamCands - 1], li[kBeamCands - 1])) continue;
 #pragma unroll
@@ -236,17 +251,32 @@ __global__ void __launch_bounds__(kBeamThreads) beam_step_kernel(const float* __
   long long* run_nxt = run_tok + (size_t)((t + 1) & 1) * rows * stride;
   const long long* fin_old = fin_tok + (size_t)(t & 1) * rows * stride;
   long long* fin_nxt = fin_tok + (size_t)((t + 1) & 1) * rows * stride;
+  const bool track = s->bidx_out != nullptr;
+  const int* run_bi_old = run_bi + (size_t)(t & 1) * rows * stride;
+  int* run_bi_nxt = run_bi + (size_t)((t + 1) & 1) * rows * stride;
+  const int* fin_bi_old = fin_bi + (size_t)(t & 1) * rows * stride;
+  int* fin_bi_nxt = fin_bi + (size_t)((t + 1) & 1) * rows * stride;
   for (int e = tid; e < 2 * nb * (t + 1); e += kBeamThreads) {
     const int which = e / (nb * (t + 1)), r = e - which * nb * (t + 1), j = r / (t + 1), p = r - j * (t + 1);
     long long v;
     if (which == 0) {
-      v = p == t ? run_new[j] : run_old[(size_t)(r0 + run_src[j]) * stride + p];
+      const int parent = r0 + run_src[j];
+      v = p == t ? run_new[j] : run_old[(size_t)parent * stride + p];
       run_nxt[(size_t)(r0 + j) * stride + p] = v;
+      if (track) run_bi_nxt[(size_t)(r0 + j) * stride + p] = p == t ? parent : run_bi_old[(size_t)parent * stride + p];
     } else {
       const int src = fin_src[j];
-      if (src >= 0) v = p == t ? (long long)(cand_i[src] % V) : run_old[(size_t)(r0 + cand_i[src] / V) * stride + p];
-      else v = fin_old[(size_t)(r0 - 1 - src) * stride + p];
+      int bi;
+      if (src >= 0) {
+        const int parent = r0 + cand_i[src] / V;
+        v = p == t ? (long long)(cand_i[src] % V) : run_old[(size_t)parent * stride + p];
+        bi = p == t ? parent : (track ? run_bi_old[(size_t)parent * stride + p] : 0);
+      } else {
+        v = fin_old[(size_t)(r0 - 1 - src) * stride + p];
+        bi = track ? fin_bi_old[(size_t)(r0 - 1 - src) * stride + p] : 0;
+      }
       fin_nxt[(size_t)(r0 + j) * stride + p] = v;
+      if (track) fin_bi_nxt[(size_t)(r0 + j) * stride + p] = bi;
     }
   }
   if (tid < nb) cur_tokens[r0 + tid] = run_new[tid];
@@ -271,16 +301,20 @@ __global__ void __launch_bounds__(kBeamThreads) beam_step_kernel(const float* __
 }
 
 // Results: for item g and j < nrs, output row g * nrs + j = finished slot j: seq_out [., n_cols] (fill beyond its length),
-// scores_out, len_out.
-__global__ void beam_output_kernel(const BeamState* s, const long long* fin_tok, int stride, int rows, int nrs, int n_cols,
-                                   long long fill, long long* seq_out, float* scores_out, int* len_out) {
+// scores_out, len_out; when recording, s->bidx_out [., n_cols] (-1 beyond its length) and *s->steps_out.
+__global__ void beam_output_kernel(const BeamState* s, const long long* fin_tok, const int* fin_bi, int stride, int rows, int nrs,
+                                   int n_cols, long long fill, long long* seq_out, float* scores_out, int* len_out) {
   const int o = blockIdx.x, g = o / nrs, j = o - g * nrs, r = g * s->nb + j;
-  const long long* src = fin_tok + (size_t)(s->step & 1) * rows * stride + (size_t)r * stride;
+  const size_t at = (size_t)(s->step & 1) * rows * stride + (size_t)r * stride;
+  const long long* src = fin_tok + at;
   const int len = s->fin_len[r];
   for (int p = threadIdx.x; p < n_cols; p += blockDim.x) seq_out[(size_t)o * n_cols + p] = p < len ? src[p] : fill;
+  if (s->bidx_out)
+    for (int p = threadIdx.x; p < n_cols; p += blockDim.x) s->bidx_out[(size_t)o * n_cols + p] = p < len ? (long long)fin_bi[at + p] : -1;
   if (threadIdx.x == 0) {
     scores_out[o] = s->fin_score[r];
     len_out[o] = len;
+    if (o == 0 && s->steps_out) *s->steps_out = s->step;
   }
 }
 

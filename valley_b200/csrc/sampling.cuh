@@ -48,6 +48,12 @@ struct SampleState {          // lives in device memory next to the KV cache; re
   const uint32_t* pause = nullptr;         // [ceil(V / 32)] bits, or null: emitting one of these tokens finishes the row
   int* ring = nullptr;                     // [kMaxSampleRows][kStopRing]: each row's latest tokens, the next at ring_n % kStopRing
   int ring_n[kMaxSampleRows] = {};
+  // recording (vly_sampling::scores_out / logits_out): caller buffers [slots][B][V] fp32, or null.  sample_filter_kernel writes
+  // slot *step - 1 (slot 0 for the first token, launched without a step counter): the score it selects from, logits / rec_temp
+  // or -inf where the filter removed the token, and the raw logit.
+  float* rec_scores = nullptr;
+  float* rec_logits = nullptr;
+  float rec_temp = 1.f;
   // the generation's progress
   int all_done = 0;           // every row has produced eos: further steps exit at once
   int steps_valid = 0;        // decode steps executed before all_done was raised (the one that raised it included)
@@ -182,6 +188,8 @@ __device__ __forceinline__ float key_score(uint32_t k) { return __uint_as_float(
 //     steps_valid.  After the persistent kernel (which counts its own steps and skips once all_done is raised) and for the
 //     first token, none of these.
 // keep_out != nullptr (vly_test_sample_filter): writes the kept mask [B, V] and nothing else.
+// A recording request (SampleState::rec_scores / rec_logits) writes its slot in the final pass over the row, where `keep` is
+// decided: the recorded -inf are exactly the tokens the draw excludes.  Nothing is recorded once all_done is raised.
 __global__ void __launch_bounds__(kFilterThreads) sample_filter_kernel(const float* __restrict__ logits, int V, SampleState* s,
                                                                        const int* seq_len, const int* step, long long* next_tokens,
                                                                        long long* out_tokens, int out_stride, int filter,
@@ -199,7 +207,8 @@ __global__ void __launch_bounds__(kFilterThreads) sample_filter_kernel(const flo
   __shared__ float sh_above;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, b = blockIdx.x;
   const bool select = keep_out == nullptr;
-  if (select && per_op && !s->enabled && s->eos < 0 && s->stop2 < 0 && s->n_stop == 0) return;   // plain greedy: the step's arg-max is the token
+  if (select && per_op && !s->enabled && s->eos < 0 && s->stop2 < 0 && s->n_stop == 0 && !s->rec_scores && !s->rec_logits)
+    return;                                         // plain greedy: the step's arg-max is the token
   if (select && s->all_done) {
     if (per_op && tid == 0) {                       // the per-op kernels keep stepping: emit pad
       next_tokens[b] = s->pad;
@@ -343,13 +352,25 @@ __global__ void __launch_bounds__(kFilterThreads) sample_filter_kernel(const flo
   const bool on = s->enabled != 0;
   const float inv_temp = s->inv_temp;
   const uint32_t k0 = s->seed_lo, k1 = s->seed_hi;
+  float* rec_s = nullptr;
+  float* rec_l = nullptr;
+  const float rec_temp = s->rec_temp;
+  if (select && (s->rec_scores || s->rec_logits)) {
+    const size_t row = ((size_t)(step ? *step - 1 : 0) * gridDim.x + b) * V;
+    if (s->rec_scores) rec_s = s->rec_scores + row;
+    if (s->rec_logits) rec_l = s->rec_logits + row;
+  }
   float bv = -INFINITY;
   int bi = 0x7fffffff;
   for (int n = tid; n < V; n += kFilterThreads) {
     const bool keep = !filter || score_key(score(n)) >= cut;
     if (!select) {
       keep_out[(size_t)b * V + n] = keep;
-    } else if (keep) {
+      continue;
+    }
+    if (rec_s) rec_s[n] = keep ? z[n] / rec_temp : -INFINITY;
+    if (rec_l) rec_l[n] = z[n];
+    if (keep) {
       const float v = on ? sample_score(z[n], inv_temp, k0, k1, n, b, pos) : z[n];
       if (v > bv) { bv = v; bi = n; }               // ascending n per thread: first maximum kept
     }

@@ -109,6 +109,48 @@ class CausalLMOutputWithPast(dict):
         return dict.__getitem__(self, k)
 
 
+class _GenerateOutput(dict):
+    """The surface of transformers' ``ModelOutput`` for generate()'s output classes: attribute, key and integer-index access.
+    Fields that are None are attributes only: ``keys()``, integer indices and ``to_tuple()`` skip them, as in transformers."""
+    _fields: Tuple[str, ...] = ()
+
+    def __init__(self, **kw):
+        unknown = set(kw) - set(self._fields)
+        if unknown:
+            raise TypeError(f"{type(self).__name__} has no field(s) {sorted(unknown)}")
+        super().__init__((k, kw[k]) for k in self._fields if kw.get(k) is not None)
+        self.__dict__.update({k: kw.get(k) for k in self._fields})
+
+    def __getitem__(self, k):
+        if isinstance(k, str):
+            return dict.__getitem__(self, k)
+        return self.to_tuple()[k]
+
+    def to_tuple(self) -> tuple:
+        return tuple(dict.__getitem__(self, k) for k in self._fields if k in self)
+
+
+class GenerateDecoderOnlyOutput(_GenerateOutput):
+    """transformers' ``GenerateDecoderOnlyOutput``: generate(return_dict_in_generate=True) with num_beams == 1."""
+    _fields = ("sequences", "scores", "logits", "attentions", "hidden_states", "past_key_values")
+
+
+class GenerateBeamDecoderOnlyOutput(_GenerateOutput):
+    """transformers' ``GenerateBeamDecoderOnlyOutput``: generate(return_dict_in_generate=True) with num_beams > 1."""
+    _fields = ("sequences", "sequences_scores", "scores", "logits", "beam_indices", "attentions", "hidden_states",
+               "past_key_values")
+
+
+def generation_output(sequences, steps: int, scores=None, logits=None, sequences_scores=None, beam_indices=None, beam=False):
+    """generate()'s output object from what a request recorded: ``scores`` / ``logits`` are buffers [>= steps, rows, V] (or
+    None when not asked for) of which the first ``steps`` slots were written; they become HF's per-step tuples (views)."""
+    per_step = lambda buf: None if buf is None else tuple(buf[i] for i in range(steps))
+    if beam:
+        return GenerateBeamDecoderOnlyOutput(sequences=sequences, sequences_scores=sequences_scores, scores=per_step(scores),
+                                             logits=per_step(logits), beam_indices=beam_indices)
+    return GenerateDecoderOnlyOutput(sequences=sequences, scores=per_step(scores), logits=per_step(logits))
+
+
 class _ShapeOnly:
     def __init__(self, shape):
         self.shape = torch.Size(shape)
@@ -741,7 +783,8 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
     def generate(self, input_ids=None, images=None, max_new_tokens: int = 1024, do_sample: bool = False,
                  temperature: float = 1.0, stopping_criteria=None, eos_token_id=_UNSET, top_k=None, top_p=None,
                  num_beams: int = 1, num_return_sequences: int = 1, length_penalty: float = 1.0, early_stopping=False,
-                 stop_strings=None, tokenizer=None, **kw):
+                 stop_strings=None, tokenizer=None, return_dict_in_generate: bool = False, output_scores: bool = False,
+                 output_logits: bool = False, output_attentions: bool = False, output_hidden_states: bool = False, **kw):
         """Greedy (or temperature) generation == the loop of model_worker.py:371-397 / HF generate as called at
         valley_model.py:432.  Returns [B, S + n_new] like HF.  With no stopping criteria, decoding runs
         entirely on the device (CUDA-graph replay, no per-token host sync).  ``attention_mask`` [B, S] (left padding)
@@ -769,7 +812,21 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
         only when ``eos_token_id`` is set, as in HF; generation ends when every row has finished.  With ``num_beams == 1``, no
         other stopping criteria, at most 64 rows, at most 8 stop strings and at most 64 characters each, the matcher runs on
         the device after every token (no per-token host sync); otherwise the host-visible loops check it.  ``stop_strings``
-        without ``tokenizer`` raises HF's ``ValueError``."""
+        without ``tokenizer`` raises HF's ``ValueError``.
+
+        ``return_dict_in_generate=True`` returns HF's output object instead of the tensor: ``GenerateDecoderOnlyOutput``
+        (``num_beams == 1``) or ``GenerateBeamDecoderOnlyOutput``, with transformers 5.5's fields.  ``output_scores`` adds
+        ``scores``, one [rows, V] fp32 tensor per step run: the raw logits when not sampling; when sampling, logits /
+        temperature with -inf at every token top_k / top_p removed; for beams, each beam row's log-softmax (and
+        ``sequences_scores``).  ``output_logits`` adds the raw logits per step.  Beams always return ``beam_indices``
+        [B * num_return_sequences, L]: the cache row (item * num_beams + beam) of each token, -1 after the hypothesis ended.
+        The device routes record these inside the decode loop, with no extra host synchronisation; each requested output
+        costs steps x rows x V x 4 bytes (128 KB per row and step at V = 32,000).  ``past_key_values`` is None: the KV cache
+        goes back to the model's pool when the request ends.  ``output_attentions`` / ``output_hidden_states`` raise
+        ``NotImplementedError``.  Without ``return_dict_in_generate`` the output flags are ignored, as in HF."""
+        if output_hidden_states or output_attentions:
+            raise NotImplementedError("output_hidden_states / output_attentions are not produced by the fused kernels")
+        record = (bool(output_scores), bool(output_logits)) if return_dict_in_generate else None
         B, S = input_ids.shape
         tables = None
         if stop_strings is not None:
@@ -780,18 +837,19 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
             tables = _ss.stop_tables(_ss.clean_token_strings(tokenizer), stop_strings, self.config.vocab_size)
         if num_beams != 1:
             return self._beam_generate(input_ids, images, max_new_tokens, do_sample, stopping_criteria, eos_token_id, num_beams,
-                                       num_return_sequences, length_penalty, early_stopping, tables=tables, **kw)
+                                       num_return_sequences, length_penalty, early_stopping, tables=tables, record=record, **kw)
         greedy = (not do_sample) or temperature < 1e-4
         filters = {} if greedy else dict(zip(("top_k", "top_p"), sampling_filters(top_k, top_p)))
         n_new, eos_token_id, pad_token_id, attention_mask = self._generation_defaults(input_ids, max_new_tokens, eos_token_id, kw)
         if n_new == 0:
-            return input_ids.to(self.device)
+            seq = input_ids.to(self.device)
+            return seq if record is None else generation_output(seq, 0, *self._record_buffers(record, 0, B))
         _, _, _, embeds, _ = self.prepare_inputs_labels_for_multimodal(input_ids, None, None, None, images)
         cache = self.new_cache(B)
         try:
             cache.set_attention_mask(attention_mask, S)
             return self._generate_with_cache(cache, input_ids, embeds, n_new, do_sample, temperature, stopping_criteria, eos_token_id,
-                                             pad_token_id, tables=tables, **filters)
+                                             pad_token_id, tables=tables, record=record, **filters)
         finally:
             cache.release()
 
@@ -812,18 +870,29 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
                 attention_mask = (~is_pad).to(torch.int64)
         return n_new, eos_token_id, pad_token_id, attention_mask
 
+    def _record_buffers(self, record, n_steps: int, rows: int):
+        """(scores, logits) buffers [n_steps, rows, V] fp32 for a request that records them (``record`` = (output_scores,
+        output_logits), or None: nothing is recorded); None for an output not asked for"""
+        V = self.config.vocab_size
+        mk = lambda want: torch.empty(n_steps, rows, V, dtype=torch.float32, device=self.device) if want else None
+        return (None, None) if record is None else (mk(record[0]), mk(record[1]))
+
     def _generate_with_cache(self, cache, input_ids, embeds, n_new, do_sample, temperature, stopping_criteria, eos_token_id,
-                             pad_token_id=None, top_k=0, top_p=1.0, tables=None):
+                             pad_token_id=None, top_k=0, top_p=1.0, tables=None, record=None):
+        """the tokens after the prefill of ``embeds`` into ``cache``: [B, S + steps], or with ``record`` = (output_scores,
+        output_logits) the output object of generate(return_dict_in_generate=True)"""
         B = input_ids.shape[0]
         greedy = (not do_sample) or temperature < 1e-4
-        device_select = (not stopping_criteria and not (greedy and eos_token_id is None and tables is None) and B <= 64
+        plain = greedy and not stopping_criteria and eos_token_id is None and tables is None
+        device_select = (not stopping_criteria and not (plain and record is None) and B <= 64
                          and (tables is None or tables.on_device))
+        rec_scores, rec_logits = self._record_buffers(record, n_new, B)
         tail = None
         if device_select and tables is not None:       # the prompt's last tokens seed the device matcher (the whole row counts)
             tail = input_ids[:, -min(input_ids.shape[1], 63):].to("cpu", torch.int64).numpy()
-        logits, nxt = self._prefill(cache, embeds, 0 if (greedy and not device_select) else 1)
+        logits, nxt = self._prefill(cache, embeds, 0 if (greedy and not device_select and record is None) else 1)
         ids_dev = input_ids.to(self.device, torch.int64)
-        if greedy and not stopping_criteria and eos_token_id is None and tables is None:
+        if plain and record is None:
             out = torch.empty(B, n_new, dtype=torch.int64, device=self.device)
             out[:, 0] = nxt
             if n_new > 1:
@@ -838,9 +907,12 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
             pad = int(pad_token_id) if pad_token_id is not None else max(eos, 0)      # HF: pad defaults to eos
             seed = int(torch.randint(0, 2 ** 62, (1,)).item())                         # torch.manual_seed() governs it
             # (a top-k / top-p filter: one more kernel per step selects over the step's logits, still on the device)
-            sp = VlySampling(0.0 if greedy else float(temperature), seed, eos, pad, top_k=top_k, top_p=top_p)
+            # below a temperature of 1e-4 the library takes the arg-max; a sampling request still passes its temperature, which
+            # its recorded scores divide by (HF's warper)
+            sp = VlySampling(float(temperature) if do_sample else 0.0, seed, eos, pad, top_k=top_k, top_p=top_p)
             if tables is not None:
                 sp.set_stop_strings(tables, tail)
+            sp.scores_out, sp.logits_out = _ptr(rec_scores), _ptr(rec_logits)      # slot 0: the first token
             out = torch.empty(B, n_new, dtype=torch.int64, device=self.device)
             first = torch.empty(B, dtype=torch.int64, device=self.device)
             check(self._lib.vly_sample_logits(self._ctx, cache._h, logits.data_ptr(), C.byref(sp), first.data_ptr(), _stream()))
@@ -849,30 +921,42 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
             if n_new > 1:
                 rest = torch.empty(B, n_new - 1, dtype=torch.int64, device=self.device)
                 done = torch.zeros(1, dtype=torch.int32, device=self.device)
+                sp.scores_out = None if rec_scores is None else rec_scores[1:].data_ptr()     # step i writes slot i + 1
+                sp.logits_out = None if rec_logits is None else rec_logits[1:].data_ptr()
                 check(self._lib.vly_generate(self._ctx, cache._h, first.data_ptr(), n_new - 1, rest.data_ptr(), C.byref(sp),
                                              done.data_ptr(), _stream()))
                 out[:, 1:] = rest
-                n_valid += int(done.item())
-            return torch.cat([ids_dev, out[:, :n_valid]], dim=1)
+                # (a plain greedy request, here only because it records, runs every step: no read-back)
+                n_valid += n_new - 1 if plain else int(done.item())
+            seq = torch.cat([ids_dev, out[:, :n_valid]], dim=1)
+            return seq if record is None else generation_output(seq, n_valid, rec_scores, rec_logits)
         # host-visible loop (stopping criteria present, B > 64, or stop strings past the device limits): one device->host
         # sync per token, as in the reference
         seq = ids_dev
         finished = torch.zeros(B, dtype=torch.bool, device=self.device)
         pad = int(pad_token_id) if pad_token_id is not None else (int(eos_token_id) if eos_token_id is not None else 0)
+        steps = 0
         for i in range(n_new):
             if not greedy:
                 scores = filter_scores(logits[:, -1, :] / temperature, top_k, top_p)     # model_worker.py:393-394
                 probs = torch.softmax(scores, dim=-1)
                 nxt = torch.multinomial(probs, num_samples=1).reshape(B)
+            elif rec_scores is not None:
+                scores = logits[:, -1, :] / temperature if do_sample else logits[:, -1, :]
+            if rec_scores is not None:
+                rec_scores[i] = scores
+            if rec_logits is not None:
+                rec_logits[i] = logits[:, -1, :]
+            steps = i + 1
             seq, nxt, finished, stop = host_rows_step(seq, nxt, finished, eos_token_id, pad, tables, stopping_criteria)
             if stop:
                 break
             if i + 1 < n_new:
-                logits, nxt = self._decode(cache, nxt, not greedy)
-        return seq
+                logits, nxt = self._decode(cache, nxt, not greedy or record is not None)
+        return seq if record is None else generation_output(seq, steps, rec_scores, rec_logits)
 
     def _beam_generate(self, input_ids, images, max_new_tokens, do_sample, stopping_criteria, eos_token_id, num_beams,
-                       num_return_sequences, length_penalty, early_stopping, tables=None, **kw):
+                       num_return_sequences, length_penalty, early_stopping, tables=None, record=None, **kw):
         """generate(num_beams > 1): the vision part is encoded once per row, then every row's embeddings and attention mask
         are repeated num_beams times (HF's _expand_inputs_for_generation) and prefilled as B * num_beams cache rows."""
         if not isinstance(num_beams, int) or num_beams < 1:
@@ -888,7 +972,11 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
         n_new, eos_token_id, pad_token_id, attention_mask = self._generation_defaults(input_ids, max_new_tokens, eos_token_id, kw)
         ids_dev = input_ids.to(self.device, torch.int64)
         if n_new == 0:
-            return _repeat_rows(ids_dev, num_return_sequences)
+            seq = _repeat_rows(ids_dev, num_return_sequences)
+            if record is None:
+                return seq
+            empty = torch.empty(seq.shape[0], 0, dtype=torch.int64, device=self.device)
+            return generation_output(seq, 0, *self._record_buffers(record, 0, B * nb), beam_indices=empty, beam=True)
         fill = _beam.output_fill_value(pad_token_id, eos_token_id)
         _, _, _, embeds, _ = self.prepare_inputs_labels_for_multimodal(input_ids, None, None, None, images)
         embeds = _repeat_rows(embeds, nb)
@@ -907,14 +995,26 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
                 seq = torch.empty(B * nrs, n_new, dtype=torch.int64, device=self.device)
                 scores = torch.empty(B * nrs, dtype=torch.float32, device=self.device)
                 lens = torch.empty(B * nrs, dtype=torch.int32, device=self.device)
+                if record is not None:
+                    rec_scores, rec_logits = self._record_buffers(record, n_new, B * nb)
+                    bidx = torch.empty(B * nrs, n_new, dtype=torch.int64, device=self.device)
+                    steps = torch.empty(1, dtype=torch.int32, device=self.device)
+                    bp.scores_out, bp.logits_out = _ptr(rec_scores), _ptr(rec_logits)
+                    bp.beam_indices_out, bp.steps_out = bidx.data_ptr(), steps.data_ptr()
                 check(self._lib.vly_beam_search(self._ctx, cache._h, C.byref(bp), logits.data_ptr(), S, n_new, seq.data_ptr(),
                                                 scores.data_ptr(), lens.data_ptr(), _stream()))
-                L = int(lens.max())                          # the request's one device-to-host read
                 self.last_beam_scores = scores
-                return torch.cat([_repeat_rows(ids_dev, nrs), seq[:, :L]], dim=1)
+                if record is None:
+                    L = int(lens.max())                      # the request's one device-to-host read
+                    return torch.cat([_repeat_rows(ids_dev, nrs), seq[:, :L]], dim=1)
+                L, n_steps = torch.stack([lens.max(), steps[0]]).tolist()      # (still one read)
+                return generation_output(torch.cat([_repeat_rows(ids_dev, nrs), seq[:, :L]], dim=1), n_steps, rec_scores,
+                                         rec_logits, sequences_scores=scores if record[0] else None,
+                                         beam_indices=bidx[:, :L], beam=True)
             # host-visible loop: the same search in torch over the library's logits, with HF's stopping criteria on the
             # candidates (a criterion returning a plain bool applies to every row, as in HF's StoppingCriteriaList)
-            bs = _beam.BeamSearch(ids_rep, nb, n_new, eos_token_id, fill, length_penalty, early_stopping)
+            bs = _beam.BeamSearch(ids_rep, nb, n_new, eos_token_id, fill, length_penalty, early_stopping,
+                                  record_scores=record is not None and record[0], record_logits=record is not None and record[1])
             stop = None
             if stopping_criteria or tables is not None:
                 def stop(seqs):
@@ -932,9 +1032,38 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
                 step_logits, _ = self._decode(cache, tokens, True)
                 logits = step_logits[:, -1]
             out, self.last_beam_scores = bs.result(num_return_sequences)
-            return out
+            if record is None:
+                return out
+            stacked = lambda steps: torch.stack(steps) if steps is not None else None
+            return generation_output(out, bs.t, stacked(bs.scores), stacked(bs.logits),
+                                     sequences_scores=self.last_beam_scores if record[0] else None,
+                                     beam_indices=bs.beam_indices(num_return_sequences), beam=True)
         finally:
             cache.release()
+
+    def compute_transition_scores(self, sequences: torch.Tensor, scores, beam_indices: Optional[torch.Tensor] = None,
+                                  normalize_logits: bool = False) -> torch.Tensor:
+        """transformers' ``GenerationMixin.compute_transition_scores``: the score of each generated token of ``sequences``
+        [rows, S + L] at its step, from ``scores`` (generate's per-step tuple) and, after a beam search, ``beam_indices``;
+        [rows, L], 0 after a hypothesis ended.  ``normalize_logits`` applies a log-softmax over the vocabulary first."""
+        V = self.config.vocab_size
+        if beam_indices is None:             # greedy / sampling: row r always continues row r
+            beam_indices = torch.arange(scores[0].shape[0]).view(-1, 1).to(sequences.device)
+            beam_indices = beam_indices.expand(-1, len(scores))
+        stacked = torch.stack(scores).reshape(len(scores), -1).transpose(0, 1)       # [rows * V, steps]
+        if normalize_logits:
+            stacked = stacked.reshape(-1, V, stacked.shape[-1])
+            stacked = torch.nn.functional.log_softmax(stacked, dim=1)
+            stacked = stacked.reshape(-1, stacked.shape[-1])
+        mask = beam_indices < 0
+        max_len = (1 - mask.long()).sum(-1).max()
+        beam_indices = beam_indices.clone()[:, :max_len]
+        mask = mask[:, :max_len]
+        beam_indices[mask] = 0
+        indices = sequences[:, sequences.shape[-1] - max_len:] + beam_indices * V
+        out = stacked.gather(0, indices)
+        out[mask] = 0
+        return out
 
     _KEYWORD_ROUTE_ARGS = frozenset({"max_new_tokens", "do_sample", "temperature", "eos_token_id", "pad_token_id",
                                      "attention_mask", "top_k", "top_p", "num_beams", "use_cache"})
