@@ -225,6 +225,21 @@ typedef struct {
   int32_t stop_restart;            /* vly_generate: 1 = start the matcher here (upload the tables, seed the rows from stop_tail
                                     * and clear the finished flags); 0 = continue the request vly_sample_logits started.
                                     * vly_sample_logits always starts it. */
+  /* Logits processors (transformers 5.5's RepetitionPenaltyLogitsProcessor, NoRepeatNGramLogitsProcessor and
+   * MinLengthLogitsProcessor, in that order, before the temperature and the top-k / top-p filter), over each row's input_ids as
+   * HF holds them: the cache's tokens (prompt_ids_dev), then every emitted token (pad_token_id once the row finished).
+   *   repetition_penalty > 0: the score s of every id in the row becomes s * penalty if s < 0, else s / penalty (IEEE fp32);
+   *   no_repeat_ngram_size n > 0: every token that followed an earlier occurrence of the row's last n - 1 ids scores -inf;
+   *   min_length > 0 (with eos_token_id >= 0): eos scores -inf while the row holds fewer than min_length ids.
+   * scores_out records the processed scores (then tempered and filtered); logits_out stays raw.  The row histories live in a
+   * buffer the cache allocates on its first processor request and keeps.  A request with processors selects in the
+   * filtered-token step (one more kernel per step at B <= 4).  Zero fields (and a penalty of 1) mean off.
+   * prompt_ids_dev: device [B, cache length] int64, read when a request starts (vly_sample_logits, or stop_restart).
+   * vly_generate with processors must continue the processor request vly_sample_logits started (VLY_ERR_STATE otherwise). */
+  float repetition_penalty;
+  int32_t no_repeat_ngram_size;
+  int32_t min_length;
+  const int64_t* prompt_ids_dev;
   /* Recording (HF generate's output_scores / output_logits): device buffers [n_slots, B, V] fp32 owned by the caller, or NULL.
    * vly_sample_logits writes slot 0; vly_generate writes slot i for its step i (pass pointers offset by one slot to continue
    * the request vly_sample_logits started).  scores_out: the scores the token is selected from -- logits / temperature when
@@ -309,6 +324,11 @@ int vly_test_vit_attention(vly_ctx* ctx, const void* qkv_dev, int n_frames, void
  * computed by the same device routine the decode loop selects with.  temperature > 0; top_k / top_p as in vly_sampling. */
 int vly_test_sample_filter(vly_ctx* ctx, const float* logits_dev, int B, int V, float temperature, int top_k, float top_p,
                            uint8_t* keep_out_dev, void* stream);
+/* the logits processors of vly_sampling alone, by the device routine the decode loop selects with: out_dev [B,V] fp32 = the
+ * processed scores of logits_dev [B,V] fp32 (any V) for input_ids ids_dev [B,L] int64.  penalty > 0 (1: off), ngram >= 0
+ * (0: off), min_length >= 0 with eos (< 0: off) as in vly_sampling. */
+int vly_test_logits_process(vly_ctx* ctx, const float* logits_dev, int B, int V, const int64_t* ids_dev, int L, float penalty,
+                            int ngram, int min_length, int64_t eos, float* out_dev, void* stream);
 /* the stop-string matcher of vly_sampling alone: with the stop-string fields of `sampling` (tables over a vocabulary of V
  * tokens; the tail and pause fields are not used), out_dev[b] (uint8) = 1 when row b of tokens_dev [B, n] int64, read as a
  * row whose newest token is the last, matches.  B <= 64.  Synchronises the stream. */

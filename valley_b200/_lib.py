@@ -39,6 +39,8 @@ class VlySampling(C.Structure):
                 ("n_stop_strings", C.c_int32), ("stop_lens", C.POINTER(C.c_int32)), ("stop_masks", C.POINTER(C.c_uint64)),
                 ("stop_token_lens", C.POINTER(C.c_int32)), ("pause_bits", C.POINTER(C.c_uint32)),
                 ("stop_tail", C.POINTER(C.c_int64)), ("stop_tail_len", C.c_int32), ("stop_restart", C.c_int32),
+                ("repetition_penalty", C.c_float), ("no_repeat_ngram_size", C.c_int32), ("min_length", C.c_int32),
+                ("prompt_ids_dev", C.c_void_p),
                 ("scores_out", C.c_void_p), ("logits_out", C.c_void_p)]
 
     def __init__(self, temperature=0.0, seed=0, eos_token_id=-1, pad_token_id=0, stop_token_id=-1, top_k=0, top_p=1.0):
@@ -130,6 +132,7 @@ SIGNATURES = {
     "vly_test_gemm": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp]),
     "vly_test_vit_attention": (_i, [_vp, _vp, _i, _vp, _vp]),
     "vly_test_sample_filter": (_i, [_vp, _vp, _i, _i, C.c_float, _i, C.c_float, _vp, _vp]),
+    "vly_test_logits_process": (_i, [_vp, _vp, _i, _i, _vp, _i, C.c_float, _i, _i, _i64, _vp, _vp]),
     "vly_test_stop_strings": (_i, [_vp, _p(VlySampling), _i, _vp, _i, _i, _vp, _vp]),
     "vly_test_gemv":(_i, [_vp, _i, _vp, _vp, _i, _i, _i, _i64, C.c_float, _vp, _vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     "vly_test_decode_attention": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),

@@ -15,6 +15,8 @@ from typing import Callable, Optional
 
 import torch
 
+from . import processors as _proc
+
 NEG = -1.0e9
 
 
@@ -46,10 +48,13 @@ class BeamSearch:
     HF's loop would stop.  ``result(num_return_sequences)`` gives ``(sequences [B * nrs, S + L], sequences_scores [B * nrs])``,
     ``beam_indices(num_return_sequences)`` HF's ``beam_indices`` [B * nrs, L] next to them.  ``record_scores`` / ``record_logits``
     keep every step's log-probabilities / logits [B * num_beams, V] in ``scores`` / ``logits`` (HF's output_scores /
-    output_logits); ``t`` is the number of steps run."""
+    output_logits); ``t`` is the number of steps run.  ``processors`` (``processors.Processors``) are applied to every beam row's
+    log-probabilities with the running hypotheses as input_ids, before the beam scores are added, as HF does; the recorded
+    scores are the processed log-probabilities."""
 
     def __init__(self, prompt_ids: torch.Tensor, num_beams: int, max_new_tokens: int, eos_token_id: Optional[int], fill: int,
-                 length_penalty: float = 1.0, early_stopping=False, record_scores: bool = False, record_logits: bool = False):
+                 length_penalty: float = 1.0, early_stopping=False, record_scores: bool = False, record_logits: bool = False,
+                 processors: Optional[_proc.Processors] = None):
         rows, S = prompt_ids.shape
         self.nb, self.B, self.S, self.n_new = num_beams, rows // num_beams, S, max_new_tokens
         self.K = 2 * num_beams                     # max(2, 1 + n_eos) * num_beams with at most one eos id
@@ -71,6 +76,7 @@ class BeamSearch:
         self.scores = [] if record_scores else None
         self.logits = [] if record_logits else None
         self.t, self.done = 0, False
+        self.processors = processors
         self.margins = []                          # per step: the smallest gap between consecutive top-(K+1) candidates
 
     def _div(self, length: int) -> torch.Tensor:
@@ -81,6 +87,8 @@ class BeamSearch:
         V = logits.shape[-1]
         cur = self.S + t
         log_probs = log_softmax(logits.float())
+        if self.processors is not None:
+            log_probs = _proc.apply(log_probs, self.seq[:, :, :cur].reshape(B * nb, cur), self.processors)
         if self.scores is not None:
             self.scores.append(log_probs)
         if self.logits is not None:

@@ -250,6 +250,10 @@ struct vly_kv {
   Owned<uint8_t> stop_buf, stop_stage;
   cudaEvent_t stop_event = nullptr;
   bool stop_ready = false;            // the running request has stop strings, and its tables and rings are on the device
+  // logits processors (set_sampling), allocated on the cache's first processor request: every row's token history
+  // [B][Smax] int32 (SampleState::hist)
+  Owned<int> hist;
+  bool procs_ready = false;           // the running request has processors, and its rows' histories are on the device
   StepGraphs graphs[kStepKinds];      // (declared after the buffers they refer to: destroyed before them)
   size_t layer_stride() const { return (size_t)2 * B * ctx->cfg.num_attention_heads * Smax * 128; }
   bf16* k_layer(int l) const { return cache + (size_t)l * layer_stride(); }
@@ -1654,11 +1658,12 @@ static int launch_decode_mega(vly_ctx* c, vly_kv* kv, bool select, cudaStream_t 
   return with_bmax(kv->B, [&](auto bm) { return launch(c, decode_step_kernel<decltype(bm)::value>, l, p); });
 }
 
-// token selection over [B, V] logits (sampling.cuh), one CTA per row; the scores of a filtered row are staged in shared memory
+// token selection over [B, V] logits (sampling.cuh), one CTA per row; a filter = 1 launch (a filter, stop strings, recording or
+// logits processors) has room for a filtered row's staged scores and for the processors' two bitmaps in shared memory
 static int launch_sample_filter(vly_ctx* c, const float* logits, int B, int V, SampleState* s, const int* seq_len, const int* step,
                                 long long* next_tokens, long long* out_tokens, int out_stride, bool filter, bool per_op,
                                 uint8_t* keep_out, cudaStream_t st) {
-  const size_t smem = filter && (size_t)V * 4 <= (size_t)kFilterStageMaxBytes ? (size_t)V * 4 : 0;
+  const size_t smem = filter ? filter_stage_bytes(V) + proc_map_bytes(V) : 0;
   return launch(c, sample_filter_kernel, {dim3(B), dim3(kFilterThreads), smem, st}, logits, V, s, seq_len, step, next_tokens, out_tokens,
                 out_stride, filter ? 1 : 0, per_op ? 1 : 0, keep_out);
 }
@@ -1705,6 +1710,8 @@ __global__ void set_sample_state_kernel(SampleState* s, const SampleState r, int
     s->top_p = r.top_p; s->seed_lo = r.seed_lo; s->seed_hi = r.seed_hi; s->eos = r.eos; s->pad = r.pad; s->stop2 = r.stop2;
     s->n_stop = r.n_stop; s->stop_walk = r.stop_walk; s->stop_masks = r.stop_masks; s->tok_len = r.tok_len; s->pause = r.pause;
     s->ring = r.ring; s->rec_scores = r.rec_scores; s->rec_logits = r.rec_logits; s->rec_temp = r.rec_temp;
+    s->procs = r.procs; s->penalty = r.penalty; s->ngram = r.ngram; s->min_length = r.min_length; s->hist = r.hist;
+    s->hist_stride = r.hist_stride;
     if (reset_done) { s->all_done = 0; s->steps_valid = 0; }
   }
   if (threadIdx.x < kMaxStopStrings) s->stop_len[threadIdx.x] = r.stop_len[threadIdx.x];
@@ -1784,8 +1791,9 @@ static int set_sampling(vly_ctx* c, vly_kv* kv, const vly_sampling* sp, bool res
   SampleState r = {};
   kv->filtered = false;
   kv->recording = false;
-  const bool had_stop = kv->stop_ready;
+  const bool had_stop = kv->stop_ready, had_procs = kv->procs_ready;
   kv->stop_ready = false;
+  kv->procs_ready = false;
   if (!sp) {
     if (!kv->sample_dirty && !force) return VLY_OK;
     reset_done = true;
@@ -1807,7 +1815,26 @@ static int set_sampling(vly_ctx* c, vly_kv* kv, const vly_sampling* sp, bool res
       kv->stop_ready = true;
     }
     if (kv->B > kMaxSampleRows) return fail(VLY_ERR_INVALID, "sampling / eos bookkeeping supports at most %d sequences per cache", kMaxSampleRows);
-    const bool on = sp->temperature >= 1e-4f;         // model_worker.py:390: below that the reference takes the arg-max
+    // logits processors (zero fields: off): a request that resets seeds every row's history from its prompt ids, one that
+    // keeps the flags continues the processor request vly_sample_logits started
+    if (!(sp->repetition_penalty >= 0.f) || sp->no_repeat_ngram_size < 0 || sp->min_length < 0)
+      return fail(VLY_ERR_INVALID, "vly_sampling: repetition_penalty %g, no_repeat_ngram_size %d and min_length %d must be >= 0",
+                  (double)sp->repetition_penalty, sp->no_repeat_ngram_size, sp->min_length);
+    const float penalty = sp->repetition_penalty == 0.f ? 1.f : sp->repetition_penalty;
+    if (penalty != 1.f || sp->no_repeat_ngram_size > 0 || (sp->min_length > 0 && sp->eos_token_id >= 0)) {
+      if (!reset_done && !had_procs)
+        return fail(VLY_ERR_STATE, "vly_generate: logits processors continue a request started by vly_sample_logits");
+      const int S = kv->host_len;
+      if (reset_done && (!sp->prompt_ids_dev || S <= 0))
+        return fail(VLY_ERR_INVALID, "vly_sampling: logits processors need prompt_ids_dev [B, %d] when a request starts", S);
+      if (!kv->hist) TRY(kv->hist.alloc((size_t)kv->B * kv->Smax * sizeof(int)));
+      if (reset_done)
+        TRY(launch(c, hist_seed_kernel, {dim3(kv->B), dim3(256), 0, st}, (int*)kv->hist, kv->Smax, (const long long*)sp->prompt_ids_dev, S));
+      r.procs = 1; r.penalty = penalty; r.ngram = sp->no_repeat_ngram_size; r.min_length = sp->min_length;
+      r.hist = kv->hist; r.hist_stride = kv->Smax;
+      kv->procs_ready = true;
+    }
+    const bool on = sp->temperature >= 1e-4f;        // model_worker.py:390: below that the reference takes the arg-max
     if (on) {
       r.temperature = sp->temperature; r.inv_temp = 1.f / sp->temperature; r.enabled = 1; r.top_k = sp->top_k; r.top_p = sp->top_p;
     }
@@ -1893,7 +1920,7 @@ extern "C" int vly_sample_logits(vly_ctx* c, vly_kv* kv, const float* logits, co
   TRY(set_sampling(c, kv, sp, true, st));
   // (no step counter: the first token records into slot 0)
   return launch_sample_filter(c, logits, kv->B, c->cfg.vocab_size, kv->d_sample, kv->d_len, nullptr, (long long*)tokens_out, nullptr,
-                              0, kv->filtered, false, nullptr, st);
+                              0, kv->filtered || kv->procs_ready, false, nullptr, st);
 }
 
 static int generate_impl(vly_ctx* c, vly_kv* kv, const int64_t* first_tokens, int n_steps, int64_t* out_tokens, const vly_sampling* sp,
@@ -1922,8 +1949,10 @@ static int generate_impl(vly_ctx* c, vly_kv* kv, const int64_t* first_tokens, in
   CK(cudaMemcpyAsync(kv->cur_tokens, first_tokens, (size_t)kv->B * 8, cudaMemcpyDeviceToDevice, st));
   CK(cudaMemsetAsync(kv->d_step, 0, 4, st));
   if (steps_done_dev) CK(cudaMemsetAsync(&kv->d_sample->steps_valid, 0, 4, st));
-  // (a stop-string request selects in sample_filter_kernel, which runs the matcher; a recording one, which writes its slot)
-  TRY(run_steps(c, kv, kv->filtered || kv->stop_ready || kv->recording ? STEP_FILTERED : STEP_TOKEN, 0, n_steps, st));
+  // (a stop-string request selects in sample_filter_kernel, which runs the matcher; a recording one, which writes its slot;
+  //  one with logits processors, which applies them)
+  TRY(run_steps(c, kv, kv->filtered || kv->stop_ready || kv->recording || kv->procs_ready ? STEP_FILTERED : STEP_TOKEN, 0, n_steps,
+                st));
   if (out_tokens)
     CK(cudaMemcpy2DAsync(out_tokens, (size_t)n_steps * 8, kv->gen_tokens, (size_t)kv->Smax * 8, (size_t)n_steps * 8, kv->B,
                          cudaMemcpyDeviceToDevice, st));
@@ -2108,6 +2137,16 @@ extern "C" int vly_test_sample_filter(vly_ctx* c, const float* logits, int B, in
   TRY(ensure(c->w_score, sizeof(SampleState)));
   CK(cudaMemcpyAsync(c->w_score.p, &s, sizeof(s), cudaMemcpyHostToDevice, st));
   return launch_sample_filter(c, logits, B, V, (SampleState*)c->w_score.p, nullptr, nullptr, nullptr, nullptr, 0, true, false, keep_out, st);
+}
+
+extern "C" int vly_test_logits_process(vly_ctx* c, const float* logits, int B, int V, const int64_t* ids, int L, float penalty,
+                                       int ngram, int min_length, int64_t eos, float* out, void* stream) {
+  if (!c || !logits || !ids || !out || B <= 0 || B > 65535 || V <= 0 || L <= 0 || !(penalty > 0.f) || ngram < 0 || min_length < 0)
+    return fail(VLY_ERR_INVALID, "vly_test_logits_process: bad argument");
+  std::lock_guard<std::mutex> lk(c->mu);
+  CK(cudaSetDevice(c->cfg.device));
+  return launch(c, logits_process_test_kernel, {dim3(B), dim3(1024), proc_map_bytes(V), (cudaStream_t)stream}, logits, V,
+                (const long long*)ids, L, penalty, ngram, min_length, (long long)eos, out);
 }
 
 extern "C" int vly_test_stop_strings(vly_ctx* c, const vly_sampling* sp, int V, const int64_t* tokens, int B, int n, uint8_t* out,

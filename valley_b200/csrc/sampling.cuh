@@ -54,6 +54,15 @@ struct SampleState {          // lives in device memory next to the KV cache; re
   float* rec_scores = nullptr;
   float* rec_logits = nullptr;
   float rec_temp = 1.f;
+  // logits processors (HF's RepetitionPenalty / NoRepeatNGram / MinLength, in that order, before the temperature and the
+  // filters): procs == 0: none.  hist [B][hist_stride] int32 is each row's input_ids as HF holds them -- the prompt, seeded
+  // by set_sampling, then every token sample_filter_kernel emits (pad in a finished row), written at pos + 1.
+  int procs = 0;
+  float penalty = 1.f;        // 1: off
+  int ngram = 0;              // 0: off
+  int min_length = 0;         // eos is banned while the row is shorter; 0: off
+  int* hist = nullptr;
+  int hist_stride = 0;
   // the generation's progress
   int all_done = 0;           // every row has produced eos: further steps exit at once
   int steps_valid = 0;        // decode steps executed before all_done was raised (the one that raised it included)
@@ -152,6 +161,71 @@ __global__ void stop_match_test_kernel(const SampleState s, int V, const long lo
   if (lane == 0) out[b] = hit;
 }
 
+// ---- logits processors: HF's RepetitionPenaltyLogitsProcessor, NoRepeatNGramLogitsProcessor, MinLengthLogitsProcessor ----
+// For one row with input_ids ids[0..L) (cur_len = L) and raw scores z:
+//   penalty: every id in ids (once, however often it occurs) scores z * penalty if z < 0, else z / penalty (IEEE fp32);
+//   ngram n: for every start j <= L - n whose ids[j .. j+n-2] equal the row's last n - 1 ids, ids[j+n-1] scores -inf
+//            (nothing when L + 1 < n: no start exists; n = 1 bans every id of the row);
+//   min_length: eos scores -inf while L < min_length.
+// -inf wins over the penalty in any order, so proc_score applies all three at once.  The CTA first marks the ids in two
+// bitmaps in shared memory, `seen` (penalty) and `banned` (n-gram), with integer atomics: the maps -- and so the scores -- are
+// a deterministic function of the row.  Ids outside [0, V) mark nothing.
+struct ProcMaps {
+  uint32_t* seen;
+  uint32_t* banned;
+  float penalty;
+  long long eos_ban;          // the eos id while it is banned, else -1
+};
+
+template <typename Id>
+__device__ void proc_build_maps(const Id* ids, int L, int V, float penalty, int ngram, int min_length, long long eos,
+                                ProcMaps& m, int tid, int nthreads) {
+  const int words = (V + 31) >> 5;
+  for (int w = tid; w < words; w += nthreads) { m.seen[w] = 0u; m.banned[w] = 0u; }
+  __syncthreads();
+  if (penalty != 1.f)
+    for (int j = tid; j < L; j += nthreads) {
+      const long long t = (long long)ids[j];
+      if (t >= 0 && t < V) atomicOr(&m.seen[t >> 5], 1u << (t & 31));
+    }
+  if (ngram > 0) {
+    const Id* tail = ids + (L - ngram + 1);         // the row's last n - 1 ids
+    for (int j = tid; j + ngram <= L; j += nthreads) {
+      bool match = true;
+      for (int k = 0; k < ngram - 1 && match; ++k) match = ids[j + k] == tail[k];
+      const long long t = (long long)ids[j + ngram - 1];
+      if (match && t >= 0 && t < V) atomicOr(&m.banned[t >> 5], 1u << (t & 31));
+    }
+  }
+  __syncthreads();
+  m.penalty = penalty;
+  m.eos_ban = eos >= 0 && L < min_length ? eos : -1;
+}
+
+__device__ __forceinline__ float proc_score(const ProcMaps& m, int n, float z) {
+  const uint32_t bit = 1u << (n & 31);
+  if ((m.banned[n >> 5] & bit) || n == m.eos_ban) return -INFINITY;
+  if (m.seen[n >> 5] & bit) return z < 0.f ? z * m.penalty : z / m.penalty;
+  return z;
+}
+
+// vly_test_logits_process: one CTA per row of logits [B, V] with input_ids [B, L]: out = the processed scores
+__global__ void __launch_bounds__(1024) logits_process_test_kernel(const float* logits, int V, const long long* ids, int L,
+                                                                   float penalty, int ngram, int min_length, long long eos,
+                                                                   float* out) {
+  extern __shared__ uint32_t maps[];                // [2][ceil(V / 32)]
+  const int b = blockIdx.x;
+  ProcMaps m = {maps, maps + ((V + 31) >> 5), 1.f, -1};
+  proc_build_maps(ids + (size_t)b * L, L, V, penalty, ngram, min_length, eos, m, threadIdx.x, blockDim.x);
+  for (int n = threadIdx.x; n < V; n += blockDim.x) out[(size_t)b * V + n] = proc_score(m, n, logits[(size_t)b * V + n]);
+}
+
+// set_sampling, a request with processors that starts: hist[b][0..S) = prompt ids [B, S]
+__global__ void hist_seed_kernel(int* hist, int stride, const long long* ids, int S) {
+  const int b = blockIdx.x;
+  for (int j = threadIdx.x; j < S; j += blockDim.x) hist[(size_t)b * stride + j] = (int)ids[(size_t)b * S + j];
+}
+
 // ---- stand-alone token selection: optional top-k / top-p (nucleus) filtering, then the Gumbel-max draw ----
 // For one row, with z the fp32 logits and T the temperature:
 //   s_n = z_n / T.
@@ -171,8 +245,16 @@ __global__ void stop_match_test_kernel(const SampleState s, int V, const long lo
 // filter = 1 filters only when the request has a filter (SampleState::filter), so stop-string requests share its graphs.
 // With stop strings, warp 0 then pushes the row's token into its ring and runs stop_match_warp (sample_filter_kernel is the
 // step's selection whenever a request has stop strings).
+// With logits processors (SampleState::procs; launched with filter = 1), the CTA first builds the row's ProcMaps from
+// hist[b][0..pos], and every use of z_n as a score -- the staged scores, the draw, the recorded score -- becomes
+// proc_score(z_n); the recorded logit stays z_n.  The emitted token is written to hist[b][pos + 1].
+// Dynamic shared memory of a filter = 1 launch: the staged scores (when they fit), then the two maps.
 constexpr int kFilterThreads = 1024;
 constexpr int kFilterStageMaxBytes = 200 * 1024;     // rows of up to 51200 scores are staged
+__host__ __device__ constexpr size_t filter_stage_bytes(int V) {
+  return (size_t)V * 4 <= (size_t)kFilterStageMaxBytes ? (size_t)V * 4 : 0;
+}
+__host__ __device__ constexpr size_t proc_map_bytes(int V) { return (size_t)2 * ((V + 31) / 32) * 4; }
 
 __device__ __forceinline__ uint32_t score_key(float s) {   // unsigned order of the keys == order of the (finite) scores
   uint32_t u = __float_as_uint(s);
@@ -207,7 +289,8 @@ __global__ void __launch_bounds__(kFilterThreads) sample_filter_kernel(const flo
   __shared__ float sh_above;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, b = blockIdx.x;
   const bool select = keep_out == nullptr;
-  if (select && per_op && !s->enabled && s->eos < 0 && s->stop2 < 0 && s->n_stop == 0 && !s->rec_scores && !s->rec_logits)
+  if (select && per_op && !s->enabled && s->eos < 0 && s->stop2 < 0 && s->n_stop == 0 && !s->rec_scores && !s->rec_logits &&
+      !s->procs)
     return;                                         // plain greedy: the step's arg-max is the token
   if (select && s->all_done) {
     if (per_op && tid == 0) {                       // the per-op kernels keep stepping: emit pad
@@ -219,14 +302,22 @@ __global__ void __launch_bounds__(kFilterThreads) sample_filter_kernel(const flo
   const float temperature = s->temperature, top_p = s->top_p;
   const int top_k = s->top_k;
   const float* z = logits + (size_t)b * V;
+  const int pos = select ? *seq_len - 1 : 0;
+  const bool procs = select && filter && s->procs;
+  ProcMaps pm = {reinterpret_cast<uint32_t*>(srow + (filter ? filter_stage_bytes(V) / 4 : 0)), nullptr, 1.f, -1};
+  pm.banned = pm.seen + (V + 31) / 32;
+  if (procs)
+    proc_build_maps(s->hist + (size_t)b * s->hist_stride, pos + 1, V, s->penalty, s->ngram, s->min_length, s->eos, pm, tid,
+                    kFilterThreads);
+  auto zp = [&](int n) { return procs ? proc_score(pm, n, z[n]) : z[n]; };   // the processed score of token n
   filter = filter && (s->filter || !select);
-  const bool staged = filter && (size_t)V * 4 <= (size_t)kFilterStageMaxBytes;
-  auto score = [&](int n) { return staged ? srow[n] : z[n] / temperature; };
+  const bool staged = filter && filter_stage_bytes(V) > 0;
+  auto score = [&](int n) { return staged ? srow[n] : zp(n) / temperature; };
 
   uint32_t kmax = 0;
   if (filter) {
     for (int n = tid; n < V; n += kFilterThreads) {
-      const float sc = z[n] / temperature;
+      const float sc = zp(n) / temperature;
       if (staged) srow[n] = sc;
       kmax = max(kmax, score_key(sc));
     }
@@ -348,7 +439,6 @@ __global__ void __launch_bounds__(kFilterThreads) sample_filter_kernel(const flo
     cut = max(cut, prefix);
   }
 
-  const int pos = select ? *seq_len - 1 : 0;
   const bool on = s->enabled != 0;
   const float inv_temp = s->inv_temp;
   const uint32_t k0 = s->seed_lo, k1 = s->seed_hi;
@@ -368,10 +458,11 @@ __global__ void __launch_bounds__(kFilterThreads) sample_filter_kernel(const flo
       keep_out[(size_t)b * V + n] = keep;
       continue;
     }
-    if (rec_s) rec_s[n] = keep ? z[n] / rec_temp : -INFINITY;
+    const float zn = zp(n);
+    if (rec_s) rec_s[n] = keep ? zn / rec_temp : -INFINITY;
     if (rec_l) rec_l[n] = z[n];
     if (keep) {
-      const float v = on ? sample_score(z[n], inv_temp, k0, k1, n, b, pos) : z[n];
+      const float v = on ? sample_score(zn, inv_temp, k0, k1, n, b, pos) : zn;
       if (v > bv) { bv = v; bi = n; }               // ascending n per thread: first maximum kept
     }
   }
@@ -383,6 +474,7 @@ __global__ void __launch_bounds__(kFilterThreads) sample_filter_kernel(const flo
   bv = bv_w[lane];
   bi = bi_w[lane];
   warp_argmax(bv, bi);
+  if (procs && bi == 0x7fffffff) bi = 0;            // the processors left every score -inf: torch's argmax takes 0
   long long tok = bi;
   if (s->n_stop > 0) {
     const int was_done = s->done[b];
@@ -403,6 +495,7 @@ __global__ void __launch_bounds__(kFilterThreads) sample_filter_kernel(const flo
     if (lane != 0) return;
     tok = sample_finish_row(s, b, bi);
   }
+  if (procs && pos + 1 < s->hist_stride) s->hist[(size_t)b * s->hist_stride + pos + 1] = (int)tok;
   next_tokens[b] = tok;
   if (out_tokens) out_tokens[(size_t)b * out_stride + (*step - 1)] = tok;
   __threadfence();

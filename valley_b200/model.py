@@ -23,6 +23,7 @@ import torch
 
 from . import _lib
 from . import beam as _beam
+from . import processors as _proc
 from . import stop_strings as _ss
 from ._lib import VlyBeam, VlySampling, VlyConfig, VlyTokens, check
 
@@ -823,11 +824,20 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
         The device routes record these inside the decode loop, with no extra host synchronisation; each requested output
         costs steps x rows x V x 4 bytes (128 KB per row and step at V = 32,000).  ``past_key_values`` is None: the KV cache
         goes back to the model's pool when the request ends.  ``output_attentions`` / ``output_hidden_states`` raise
-        ``NotImplementedError``.  Without ``return_dict_in_generate`` the output flags are ignored, as in HF."""
+        ``NotImplementedError``.  Without ``return_dict_in_generate`` the output flags are ignored, as in HF.
+
+        ``repetition_penalty``, ``no_repeat_ngram_size``, ``min_new_tokens`` and ``min_length`` add transformers 5.5's logits
+        processors, under HF's conditions and with HF's errors (``valley_b200/processors.py``), before the temperature and the
+        filters; the min-length ones only with an eos id, ``min_new_tokens`` winning over ``min_length``.  They see each row as HF
+        does: the prompt ids (padding and image placeholders included), then every emitted token, pad once the row finished.
+        ``scores`` records the processed scores; ``logits`` stays raw.  With ``num_beams == 1`` they run on the device inside
+        the selection kernel, with no extra host synchronisation; beams with processors run the host beam loop, on each beam
+        row's log-softmax.  Other HF processors (``bad_words_ids``, ``suppress_tokens``, ...) are still ignored."""
         if output_hidden_states or output_attentions:
             raise NotImplementedError("output_hidden_states / output_attentions are not produced by the fused kernels")
         record = (bool(output_scores), bool(output_logits)) if return_dict_in_generate else None
         B, S = input_ids.shape
+        procs = _proc.from_kwargs(kw, S, getattr(self.config, "eos_token_id", None) if eos_token_id is _UNSET else eos_token_id)
         tables = None
         if stop_strings is not None:
             if tokenizer is None:
@@ -837,7 +847,8 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
             tables = _ss.stop_tables(_ss.clean_token_strings(tokenizer), stop_strings, self.config.vocab_size)
         if num_beams != 1:
             return self._beam_generate(input_ids, images, max_new_tokens, do_sample, stopping_criteria, eos_token_id, num_beams,
-                                       num_return_sequences, length_penalty, early_stopping, tables=tables, record=record, **kw)
+                                       num_return_sequences, length_penalty, early_stopping, tables=tables, record=record,
+                                       procs=procs, **kw)
         greedy = (not do_sample) or temperature < 1e-4
         filters = {} if greedy else dict(zip(("top_k", "top_p"), sampling_filters(top_k, top_p)))
         n_new, eos_token_id, pad_token_id, attention_mask = self._generation_defaults(input_ids, max_new_tokens, eos_token_id, kw)
@@ -849,7 +860,7 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
         try:
             cache.set_attention_mask(attention_mask, S)
             return self._generate_with_cache(cache, input_ids, embeds, n_new, do_sample, temperature, stopping_criteria, eos_token_id,
-                                             pad_token_id, tables=tables, record=record, **filters)
+                                             pad_token_id, tables=tables, record=record, procs=procs, **filters)
         finally:
             cache.release()
 
@@ -878,20 +889,21 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
         return (None, None) if record is None else (mk(record[0]), mk(record[1]))
 
     def _generate_with_cache(self, cache, input_ids, embeds, n_new, do_sample, temperature, stopping_criteria, eos_token_id,
-                             pad_token_id=None, top_k=0, top_p=1.0, tables=None, record=None):
+                             pad_token_id=None, top_k=0, top_p=1.0, tables=None, record=None, procs=None):
         """the tokens after the prefill of ``embeds`` into ``cache``: [B, S + steps], or with ``record`` = (output_scores,
-        output_logits) the output object of generate(return_dict_in_generate=True)"""
+        output_logits) the output object of generate(return_dict_in_generate=True); ``procs``: the request's logits processors
+        (``processors.Processors``) or None"""
         B = input_ids.shape[0]
         greedy = (not do_sample) or temperature < 1e-4
-        plain = greedy and not stopping_criteria and eos_token_id is None and tables is None
+        plain = greedy and not stopping_criteria and eos_token_id is None and tables is None and procs is None
         device_select = (not stopping_criteria and not (plain and record is None) and B <= 64
                          and (tables is None or tables.on_device))
         rec_scores, rec_logits = self._record_buffers(record, n_new, B)
         tail = None
         if device_select and tables is not None:       # the prompt's last tokens seed the device matcher (the whole row counts)
             tail = input_ids[:, -min(input_ids.shape[1], 63):].to("cpu", torch.int64).numpy()
-        logits, nxt = self._prefill(cache, embeds, 0 if (greedy and not device_select and record is None) else 1)
-        ids_dev = input_ids.to(self.device, torch.int64)
+        logits, nxt = self._prefill(cache, embeds, 0 if (greedy and not device_select and record is None and procs is None) else 1)
+        ids_dev = input_ids.to(self.device, torch.int64).contiguous()
         if plain and record is None:
             out = torch.empty(B, n_new, dtype=torch.int64, device=self.device)
             out[:, 0] = nxt
@@ -913,6 +925,9 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
             if tables is not None:
                 sp.set_stop_strings(tables, tail)
             sp.scores_out, sp.logits_out = _ptr(rec_scores), _ptr(rec_logits)      # slot 0: the first token
+            if procs is not None:       # (the rows' histories start from the prompt ids, on the device)
+                sp.repetition_penalty, sp.no_repeat_ngram_size = procs.penalty, procs.ngram
+                sp.min_length, sp.prompt_ids_dev = procs.min_length, ids_dev.data_ptr()
             out = torch.empty(B, n_new, dtype=torch.int64, device=self.device)
             first = torch.empty(B, dtype=torch.int64, device=self.device)
             check(self._lib.vly_sample_logits(self._ctx, cache._h, logits.data_ptr(), C.byref(sp), first.data_ptr(), _stream()))
@@ -926,8 +941,10 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
                 check(self._lib.vly_generate(self._ctx, cache._h, first.data_ptr(), n_new - 1, rest.data_ptr(), C.byref(sp),
                                              done.data_ptr(), _stream()))
                 out[:, 1:] = rest
-                # (a plain greedy request, here only because it records, runs every step: no read-back)
-                n_valid += n_new - 1 if plain else int(done.item())
+                # (a greedy request without eos or stop strings -- here because it records or has processors -- runs every
+                #  step: no read-back)
+                runs_all = greedy and eos_token_id is None and tables is None
+                n_valid += n_new - 1 if runs_all else int(done.item())
             seq = torch.cat([ids_dev, out[:, :n_valid]], dim=1)
             return seq if record is None else generation_output(seq, n_valid, rec_scores, rec_logits)
         # host-visible loop (stopping criteria present, B > 64, or stop strings past the device limits): one device->host
@@ -937,12 +954,17 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
         pad = int(pad_token_id) if pad_token_id is not None else (int(eos_token_id) if eos_token_id is not None else 0)
         steps = 0
         for i in range(n_new):
+            # the processors (before the temperature and the filters, as in HF) see the row so far
+            proc = None if logits is None else _proc.apply(logits[:, -1, :], seq, procs)
             if not greedy:
-                scores = filter_scores(logits[:, -1, :] / temperature, top_k, top_p)     # model_worker.py:393-394
+                scores = filter_scores(proc / temperature, top_k, top_p)     # model_worker.py:393-394
                 probs = torch.softmax(scores, dim=-1)
                 nxt = torch.multinomial(probs, num_samples=1).reshape(B)
-            elif rec_scores is not None:
-                scores = logits[:, -1, :] / temperature if do_sample else logits[:, -1, :]
+            else:
+                if procs is not None:
+                    nxt = proc.argmax(-1)                   # (the first maximum, as on the device)
+                if rec_scores is not None:
+                    scores = proc / temperature if do_sample else proc
             if rec_scores is not None:
                 rec_scores[i] = scores
             if rec_logits is not None:
@@ -952,11 +974,11 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
             if stop:
                 break
             if i + 1 < n_new:
-                logits, nxt = self._decode(cache, nxt, not greedy or record is not None)
+                logits, nxt = self._decode(cache, nxt, not greedy or record is not None or procs is not None)
         return seq if record is None else generation_output(seq, steps, rec_scores, rec_logits)
 
     def _beam_generate(self, input_ids, images, max_new_tokens, do_sample, stopping_criteria, eos_token_id, num_beams,
-                       num_return_sequences, length_penalty, early_stopping, tables=None, record=None, **kw):
+                       num_return_sequences, length_penalty, early_stopping, tables=None, record=None, procs=None, **kw):
         """generate(num_beams > 1): the vision part is encoded once per row, then every row's embeddings and attention mask
         are repeated num_beams times (HF's _expand_inputs_for_generation) and prefilled as B * num_beams cache rows."""
         if not isinstance(num_beams, int) or num_beams < 1:
@@ -988,7 +1010,7 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
             cache.set_attention_mask(attention_mask, S)
             logits, _ = self._prefill(cache, embeds, 1)
             logits = logits[:, -1].contiguous()
-            if not stopping_criteria and tables is None and nb <= 8 and B * nb <= 64:
+            if not stopping_criteria and tables is None and procs is None and nb <= 8 and B * nb <= 64:
                 nrs = num_return_sequences
                 es = {False: 0, True: 1, "never": 2}[early_stopping]
                 bp = VlyBeam(nb, nrs, float(length_penalty), es, -1 if eos_token_id is None else int(eos_token_id), fill)
@@ -1014,7 +1036,8 @@ class ValleyLlamaForCausalLM(_ModuleSurface):
             # host-visible loop: the same search in torch over the library's logits, with HF's stopping criteria on the
             # candidates (a criterion returning a plain bool applies to every row, as in HF's StoppingCriteriaList)
             bs = _beam.BeamSearch(ids_rep, nb, n_new, eos_token_id, fill, length_penalty, early_stopping,
-                                  record_scores=record is not None and record[0], record_logits=record is not None and record[1])
+                                  record_scores=record is not None and record[0], record_logits=record is not None and record[1],
+                                  processors=procs)
             stop = None
             if stopping_criteria or tables is not None:
                 def stop(seqs):
