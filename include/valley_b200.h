@@ -315,9 +315,33 @@ int vly_kv_debug_counters(vly_kv* kv, long long* host_out, int n);
 void vly_set_error_(const char* message);
 
 /* ---- low-level op hooks (per-kernel parity tests; SURVEY section 4) ----
- * D[M,N] = epilogue(A[M,K] * W[N,K]^T): epi 0 bias->bf16, 3 bias+residual (in-place allowed)->bf16.  bias_dev fp32 or NULL. */
+ * One prefill / ViT GEMM through the launcher production uses: acc[M,N] = A[M,K] * W[N,K]^T (bf16, K a multiple of 8, fp32
+ * accumulation) in 128 x block_n tiles (block_n 128 or 256), then the fused epilogue epi.  bias_dev / colsum_dev are fp32 [N].
+ * The normalising epilogues (1, 2, 4, 5, 6) read stats_in_dev [M, stats_in_nt] float2 partial (sum, sumsq) of the rows of A
+ * and form mean = sum / K, rstd = 1 / sqrt(sumsq / K - mean^2 + eps) (LayerNorm) or rstd = 1 / sqrt(sumsq / K + eps) (RMSNorm).
+ *   0 bias:                 out [M,N] bf16 = acc (+ bias)
+ *   1 LayerNorm + bias:     out [M,N] bf16 = rstd * (acc - mean * colsum) + bias
+ *   2 ... + quick_gelu:     out [M,N] bf16 = quick_gelu(rstd * (acc - mean * colsum) + bias)
+ *   3 bias + residual:      out [M,N] bf16 = acc (+ bias) + residual_dev [M,N] (in place allowed), N a multiple of 32;
+ *                           stats_out_dev (or NULL) [M, ceil(N / block_n)] float2 = per-tile (sum, sumsq) of the bf16 outputs
+ *   4 RMSNorm + QKV + RoPE: rows [q | k | v] of nH = N / 384 heads in pair-interleaved RoPE order; row m of A is token
+ *                           (b = m / S, s = m % S) at position past + s (M a multiple of S, past + S <= Smax <=
+ *                           max_position_embeddings); rstd * acc rotated by the context's RoPE table: q -> out [M, N/3],
+ *                           k / v -> row past + s of kcache_dev / vcache_dev [M/S, nH, Smax, 128]
+ *   5 RMSNorm + SwiGLU:     columns (2j, 2j+1) = (gate j, up j), N a multiple of 32: out [M, N/2] bf16 = silu(g) * u with
+ *                           g = rstd * acc[2j], u = rstd * acc[2j+1] (neither rounded to bf16)
+ *   6 RMSNorm, fp32:        out [M,N] fp32 = rstd * acc
+ * Arguments an epilogue does not use may be NULL / 0. */
 int vly_test_gemm(vly_ctx* ctx, const void* a_dev, const void* w_dev, int M, int N, int K, int epi, const float* bias_dev,
-                  const void* residual_dev, void* out_dev, int block_n, void* stream);
+                  const void* residual_dev, void* out_dev, int block_n, const float* colsum_dev, const void* stats_in_dev,
+                  int stats_in_nt, float eps, void* stats_out_dev, void* kcache_dev, void* vcache_dev, int S, int past, int Smax,
+                  void* stream);
+/* one layer's causal prefill attention, through the launcher the prefill uses: q_dev [B*S, nH*128] bf16 (RoPE pair-interleaved
+ * like the cache's keys), kcache_dev / vcache_dev [B, nH, Smax, 128] bf16 (Smax a multiple of 128) holding keys [0, past + S),
+ * key_mask_dev [B, past + S] uint8 (0 = key never attended) or NULL -> out_dev [B*S, nH*128] bf16: query s of row b, at position
+ * past + s, = softmax(q k^T / sqrt(128)) v over the attended keys at positions <= past + s (0 when none is attended). */
+int vly_test_prefill_attention(vly_ctx* ctx, const void* q_dev, const void* kcache_dev, const void* vcache_dev, int B, int S,
+                               int past, int nH, int Smax, const uint8_t* key_mask_dev, void* out_dev, void* stream);
 /* ViT attention on a packed qkv [F*257, 3072] bf16 -> ctx [F*257,1024] bf16 */
 int vly_test_vit_attention(vly_ctx* ctx, const void* qkv_dev, int n_frames, void* out_dev, void* stream);
 /* the top-k / top-p filter of vly_sampling over logits [B,V] fp32 (any V): keep_out [B,V] uint8 = 1 where the token is kept,

@@ -35,7 +35,8 @@ def stage_gemm():
         w = (torch.randn(N, K, device=dev) * 0.05).bfloat16()
         bias = torch.randn(N, device=dev)
         out = torch.zeros(M, N, device=dev, dtype=torch.bfloat16)
-        _lib.check(lib.vly_test_gemm(m._ctx, a.data_ptr(), w.data_ptr(), M, N, K, 0, bias.data_ptr(), None, out.data_ptr(), bn, 0))
+        _lib.check(lib.vly_test_gemm(m._ctx, a.data_ptr(), w.data_ptr(), M, N, K, 0, bias.data_ptr(), None, out.data_ptr(), bn,
+                                     None, None, 0, 0.0, None, None, None, 0, 0, 0, None))
         torch.cuda.synchronize()
         ref = a.float() @ w.float().T + bias
         err = Hh.rel_fro(out, ref)
@@ -49,7 +50,8 @@ def stage_gemm():
         if N % 32 == 0:
             res = (torch.randn(M, N, device=dev)).bfloat16()
             out2 = res.clone()
-            _lib.check(lib.vly_test_gemm(m._ctx, a.data_ptr(), w.data_ptr(), M, N, K, 3, bias.data_ptr(), out2.data_ptr(), out2.data_ptr(), bn, 0))
+            _lib.check(lib.vly_test_gemm(m._ctx, a.data_ptr(), w.data_ptr(), M, N, K, 3, bias.data_ptr(), out2.data_ptr(), out2.data_ptr(), bn,
+                                         None, None, 0, 0.0, None, None, None, 0, 0, 0, None))
             torch.cuda.synchronize()
             ref2 = ref + res.float()
             err2 = Hh.rel_fro(out2, ref2)

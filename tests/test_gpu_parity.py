@@ -41,34 +41,36 @@ def check_close(got, ref_fp32, ref_bf16=None, what=""):
     return e
 
 
-@pytest.mark.parametrize("M,N,K,bn", [(128, 128, 64, 128), (300, 512, 256, 256), (1000, 1024, 640, 256), (77, 1032, 512, 128),
-                                      (1, 256, 64, 256), (2056, 1024, 4096, 256)])
-def test_gemm_bias_and_residual(M, N, K, bn):
-    _, _, m = get("tiny")
-    a = (torch.randn(M, K, device="cuda") * 0.5).bfloat16()
-    w = (torch.randn(N, K, device="cuda") * 0.05).bfloat16()
-    bias = torch.randn(N, device="cuda")
-    out = torch.zeros(M, N, device="cuda", dtype=torch.bfloat16)
-    _lib.check(m._lib.vly_test_gemm(m._ctx, a.data_ptr(), w.data_ptr(), M, N, K, 0, bias.data_ptr(), None, out.data_ptr(), bn, 0))
-    ref = a.float() @ w.float().T + bias
-    assert Hh.rel_fro(out, ref) < 4e-3
-    if N % 32 == 0:
-        res = torch.randn(M, N, device="cuda").bfloat16()
-        out2 = res.clone()
-        _lib.check(m._lib.vly_test_gemm(m._ctx, a.data_ptr(), w.data_ptr(), M, N, K, 3, bias.data_ptr(), out2.data_ptr(), out2.data_ptr(), bn, 0))
-        assert Hh.rel_fro(out2, ref + res.float()) < 4e-3
-
-
 @pytest.mark.parametrize("F", [1, 2, 37])
 def test_vit_attention_kernel(F):
+    """vit_attention_kernel (CLIP ViT-L/14 self-attention: 257 tokens, 16 heads x 64, no mask) on a packed qkv [F*257, 3072]
+    against the float64 softmax(q k^T / 8) v of each frame: every frame attends its own 257 keys only.  The last query tile
+    (rows 256..319) spans into the next frame, and its last K/V tile reads the next frame's rows: those keys must be masked.
+    Bound: test_gpu_prefill_per_op._flash_ref with d = 64 (BF sum p |v| / sum p for the bf16 P, not BF |ref|).  Negative
+    control: the last query row also sees key 257, the next frame's first token (F >= 2).  Two identical calls give identical
+    bits."""
+    from test_gpu_prefill_per_op import _excess, _flash_ref, _note, _report
     _, _, m = get("tiny")
-    qkv = torch.randn(F * 257, 3072, device="cuda").bfloat16()
-    out = torch.zeros(F * 257, 1024, device="cuda", dtype=torch.bfloat16)
+    qkv = torch.randn(F * 257, 3072, generator=torch.Generator(device="cuda").manual_seed(200 + F), device="cuda").bfloat16()
+    out = torch.full((F * 257, 1024), float("nan"), device="cuda", dtype=torch.bfloat16)
     _lib.check(m._lib.vly_test_vit_attention(m._ctx, qkv.data_ptr(), F, out.data_ptr(), 0))
-    x = qkv.float().view(F, 257, 3, 16, 64)
-    q, k, v = (x[:, :, i].transpose(1, 2) for i in range(3))
-    ref = (torch.softmax(q @ k.transpose(-1, -2) * 0.125, -1) @ v).transpose(1, 2).reshape(F * 257, 1024)
-    assert Hh.rel_fro(out, ref) < 6e-3
+    torch.cuda.synchronize()
+    x = qkv.double().view(F, 257, 3, 16, 64)
+    every = torch.ones(1, 257, 257, dtype=torch.bool, device="cuda")
+    for f in range(F):
+        q, k, v = (x[f, :, j].transpose(0, 1) for j in range(3))                 # [16 heads, 257, 64]
+        ref, tol, _ = _flash_ref(q, k, v, every, 0.125, 64 // 16 + 4, 5)
+        got = out.view(F, 257, 16, 64)[f].transpose(0, 1)
+        _note("vit_attention", got, ref, tol)
+        if f + 1 < F:
+            k2, v2 = torch.cat([k, x[f + 1, :1, 1].transpose(0, 1)], 1), torch.cat([v, x[f + 1, :1, 2].transpose(0, 1)], 1)
+            bad, _, _ = _flash_ref(q[:, 256:], k2, v2, torch.ones(1, 1, 258, dtype=torch.bool, device="cuda"), 0.125, 8, 5)
+            assert _excess(got[:, 256:], bad, tol[:, 256:]) > 0, f
+    again = torch.empty_like(out)
+    _lib.check(m._lib.vly_test_vit_attention(m._ctx, qkv.data_ptr(), F, again.data_ptr(), 0))
+    torch.cuda.synchronize()
+    assert torch.equal(again, out)
+    _report("vit_attention")
 
 
 @pytest.mark.parametrize("spec_name,F,sel", [("tiny", 1, -2), ("tiny", 5, -1), ("tiny", 3, 0), ("tiny-wide", 8, -2)])
@@ -673,6 +675,97 @@ def test_cache_capacity_is_enforced():
     m(input_ids=ids.cuda(), past_key_values=cache)
     with pytest.raises(ValueError):
         m(input_ids=ids.cuda(), past_key_values=cache)            # 2 x 327 > 384
+
+
+@pytest.mark.parametrize("spec_name,B,pads", [("tiny", 1, None), ("tiny", 2, None), ("tiny", 3, (0, 70, 5)), ("shape-13b-1l", 2, None)])
+def test_prefill_on_a_non_empty_cache_vs_oracle(spec_name, B, pads):
+    """Prefill with past > 0: the multimodal prompt as a first forward, then the rest of the text as further multi-token
+    forward(input_ids=chunk, past_key_values=cache) calls -- a 70-token chunk that starts mid-64-block, one token passed as
+    inputs_embeds (S = 1 without input_ids takes the prefill path), a 5-token chunk -- and 3 teacher-forced decode steps, all
+    against the oracle with its own KVCache.  The QKV epilogue writes positions past + s and the causal attention starts its
+    query tiles at past + 64 qt.  With pads the batch is left-padded (70 keys: a whole 64-key block) and every call passes
+    attention_mask [B, past + S].  Logits at every position of each chunk (check_close, safe-margin arg-max), the layer-0 KV
+    cache after the chunks.  shape-13b-1l: one decoder layer at 13B widths, the oracle in fp32 on the GPU with TF32 off."""
+    spec = syn.SPECS[spec_name]
+    big = spec.hidden_size > 1024
+    if big:
+        sd = Hh.bf16_weights(spec, 2)
+        m = Hh.build_model(spec, sd)
+    else:
+        spec, sd, m = get(spec_name)
+    cfg, tok = Hh.oracle_cfg(spec), Hh.oracle_tok(spec)
+    dev = "cuda" if big else "cpu"
+    ids, px = syn.make_prompt_ids(spec, B, 2, 1, len_a=12, len_b=7), syn.make_pixels(B, 2, 1)
+    am = None
+    if pads is not None:
+        P = max(pads)
+        fill = torch.randint(3, spec.vocab_size - 8, (B, P), generator=torch.Generator().manual_seed(5))
+        ids, am = torch.cat([fill, ids], 1), torch.ones(B, P + ids.shape[1], dtype=torch.int64)
+        for b, p in enumerate(pads):
+            ids[b, :p] = 0
+            am[b, :p] = 0
+    gen = torch.Generator().manual_seed(6)
+    chunks = [torch.randint(3, spec.vocab_size - 8, (B, n), generator=gen) for n in (70, 1, 5)]
+    assert ids.shape[1] % 64 != 0                        # the first chunk starts mid-block
+    tf32 = (torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32)
+    torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
+    try:
+        with torch.no_grad():
+            w = {k: v.to(dev) for k, v in sd.items()}
+            ocache = O.KVCache(spec.num_hidden_layers)
+            mask = None if am is None else am.to(dev)
+            O.causal_lm_forward(w, cfg, tok, ids.to(dev), px.to(dev), ocache, attention_mask=mask)
+            refs = []
+            for c in chunks:
+                if mask is not None:
+                    mask = torch.cat([mask, torch.ones(B, c.shape[1], dtype=mask.dtype, device=dev)], 1)
+                refs.append(O.causal_lm_forward(w, cfg, tok, c.to(dev), None, ocache, attention_mask=mask).float().cpu())
+            ok, ov = ocache.k[0].float().cpu(), ocache.v[0].float().cpu()
+            steps, cur = [], refs[-1][:, -1].argmax(-1)
+            for i in range(3):
+                if mask is not None:
+                    mask = torch.cat([mask, torch.ones(B, 1, dtype=mask.dtype, device=dev)], 1)
+                lg = O.causal_lm_forward(w, cfg, tok, cur[:, None].to(dev), None, ocache, attention_mask=mask)[:, -1].float().cpu()
+                steps.append((cur, lg))
+                cur = lg.argmax(-1)
+            del w
+    finally:
+        torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32 = tf32
+    cache = m.new_cache(B)
+    mask = None if am is None else am.cuda()
+    m(input_ids=ids.cuda(), images=px.cuda(), past_key_values=cache, attention_mask=mask)
+    embed = sd["model.embed_tokens.weight"]
+
+    def compare(got, ref, what):
+        check_close(got, ref, None, what)
+        max_err = (got.cpu() - ref).abs().max().item()
+        top2 = ref.topk(2, -1).values
+        safe = (top2[..., 0] - top2[..., 1]) > 2 * max_err
+        assert safe.numel() < 20 or safe.float().mean() > 0.5, what
+        assert torch.equal(got.argmax(-1).cpu()[safe], ref.argmax(-1)[safe]), what
+
+    for i, (c, ref) in enumerate(zip(chunks, refs)):
+        past = cache.get_seq_length()
+        if mask is not None:
+            mask = torch.cat([mask, torch.ones(B, c.shape[1], dtype=mask.dtype, device="cuda")], 1)
+        if c.shape[1] == 1:
+            out = m(inputs_embeds=embed[c].cuda(), past_key_values=cache, attention_mask=mask)
+        else:
+            out = m(input_ids=c.cuda(), past_key_values=cache, attention_mask=mask)
+        assert out.logits.shape == ref.shape and cache.get_seq_length() == past + c.shape[1]
+        compare(out.logits, ref, f"chunk {i} (past {past}, S {c.shape[1]})")
+    k, v = cache.to_hf(0)
+    assert Hh.rel_fro(k, ok) < 2e-2 and Hh.rel_fro(v, ov) < 2e-2
+    logs, want = [], []
+    for cur, lg in steps:
+        if mask is not None:
+            mask = torch.cat([mask, torch.ones(B, 1, dtype=mask.dtype, device="cuda")], 1)
+        logs.append(m(input_ids=cur[:, None].cuda(), past_key_values=cache, attention_mask=mask).logits[:, -1])
+        want.append(lg)
+    compare(torch.stack(logs, 1), torch.stack(want, 1), "decode steps")
+    if big:
+        del m
+        torch.cuda.empty_cache()
 
 
 @pytest.mark.parametrize("spec_name,B", [("shape-13b-1l", 1), ("shape-13b-1l", 4), ("shape-7b-1l", 3), ("shape-13b-1l", 5),

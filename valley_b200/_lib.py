@@ -129,7 +129,9 @@ SIGNATURES = {
     "vly_num_sms": (_i, [_vp, _p(_i)]),
     "vly_kv_debug_counters": (_i, [_vp, _vp, _i]),
     "vly_set_error_": (None, [C.c_char_p]),
-    "vly_test_gemm": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp]),
+    "vly_test_gemm": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _i, _vp, _vp, _i, C.c_float, _vp, _vp, _vp, _i, _i, _i,
+                           _vp]),
+    "vly_test_prefill_attention": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "vly_test_vit_attention": (_i, [_vp, _vp, _i, _vp, _vp]),
     "vly_test_sample_filter": (_i, [_vp, _vp, _i, _i, C.c_float, _i, C.c_float, _vp, _vp]),
     "vly_test_logits_process": (_i, [_vp, _vp, _i, _i, _vp, _i, C.c_float, _i, _i, _i64, _vp, _vp]),

@@ -173,8 +173,9 @@ struct vly_ctx {
   Mem w_strip, w_tables;
   int pre_H = 0, pre_W = 0;
   PreprocParams pre = {};
-  // per-kernel test hooks: device scalars, work counters and partials of vly_test_gemv / vly_test_decode_attention
-  Mem w_tgemv, w_tattn;
+  // per-kernel test hooks: device scalars, work counters and partials of vly_test_gemv / vly_test_decode_attention; the packed
+  // key bits of vly_test_prefill_attention
+  Mem w_tgemv, w_tattn, w_tprefill;
 
   // (runs before the members above are freed)
   ~vly_ctx() {
@@ -1553,18 +1554,20 @@ static int launch_logits_gemv(vly_ctx* c, vly_kv* kv, int b0, int nb, const bf16
 // ------------------------------------------------------------------------------------------------
 // prefill
 // ------------------------------------------------------------------------------------------------
-static int launch_prefill_attention(vly_ctx* c, vly_kv* kv, const bf16* qbuf, int B, int S, int past, int layer, bf16* out, cudaStream_t st) {
-  const vly_config& g = c->cfg;
-  const int H = g.hidden_size, nH = g.num_attention_heads;
+// One layer's causal prefill attention: q [B*S, nH*128] against the K/V rows [0, past + S) of kcache / vcache [B, nH, Smax, 128];
+// key_bits [B, Smax/32] (1 = attend) or NULL when no key is masked.
+static int launch_prefill_attention(vly_ctx* c, const bf16* qbuf, const bf16* kcache, const bf16* vcache, int Smax, const uint32_t* key_bits,
+                                    int B, int S, int past, int nH, bf16* out, cudaStream_t st) {
+  const int H = nH * 128;
   using C = FlashCfg<128>;
   CUtensorMap tq, tk, tv;
   TRY(make_tmap_2d(c, &tq, qbuf, H, (uint64_t)B * S, (uint64_t)H * 2, 64, 64));
-  TRY(make_tmap_3d(c, &tk, kv->k_layer(layer), 128, kv->Smax, (uint64_t)B * nH, 256, (uint64_t)kv->Smax * 256, 64, 64));
-  TRY(make_tmap_3d(c, &tv, kv->v_layer(layer), 128, kv->Smax, (uint64_t)B * nH, 256, (uint64_t)kv->Smax * 256, 64, 64));
+  TRY(make_tmap_3d(c, &tk, kcache, 128, Smax, (uint64_t)B * nH, 256, (uint64_t)Smax * 256, 64, 64));
+  TRY(make_tmap_3d(c, &tv, vcache, 128, Smax, (uint64_t)B * nH, 256, (uint64_t)Smax * 256, 64, 64));
   PrefillAttnParams p;
-  p.B = B; p.S = S; p.past = past; p.nH = nH; p.H = H; p.Smax = kv->Smax; p.ctx = out;
+  p.B = B; p.S = S; p.past = past; p.nH = nH; p.H = H; p.Smax = Smax; p.ctx = out;
   p.scale_log2e = 0.08838834764831845f * 1.4426950408889634f;
-  p.key_bits = kv->masked ? static_cast<uint32_t*>(kv->key_bits) : nullptr; p.mask_words = kv->mask_words();
+  p.key_bits = key_bits; p.mask_words = Smax / 32;
   const int n_qt = cdiv(S, 64);
   return launch(c, llama_prefill_attention_kernel, {dim3(B * nH * n_qt), dim3(C::THREADS), C::SMEM_BYTES, st, true}, tq, tk, tv, p);
 }
@@ -1603,7 +1606,8 @@ extern "C" int vly_llama_prefill(vly_ctx* c, vly_kv* kv, const void* inputs_embe
       p.kcache = kv->k_layer(l); p.vcache = kv->v_layer(l);
       TRY(launch_gemm<EPI_RMS_QKV_ROPE>(c, pick_bn_m(c, 3 * H, M), x, H, w.wqkv, H, p, st));
     }
-    TRY(launch_prefill_attention(c, kv, qb, B, S, past, l, attn, st));
+    TRY(launch_prefill_attention(c, qb, kv->k_layer(l), kv->v_layer(l), kv->Smax, kv->masked ? static_cast<uint32_t*>(kv->key_bits) : nullptr,
+                                 B, S, past, nH, attn, st));
     {
       GemmParams p = {};
       p.M = M; p.N = H; p.K = H; p.out = x; p.ldo = H; p.residual = x; p.ldr = H; p.stats_out = stats;
@@ -2102,20 +2106,66 @@ extern "C" int vly_preprocess_frames(vly_ctx* c, const uint8_t* frames, int T, i
 // per-kernel test hooks
 // ------------------------------------------------------------------------------------------------
 extern "C" int vly_test_gemm(vly_ctx* c, const void* a, const void* w, int M, int N, int K, int epi, const float* bias, const void* residual,
-                             void* out, int block_n, void* stream) {
+                             void* out, int block_n, const float* colsum, const void* stats_in, int stats_in_nt, float eps, void* stats_out,
+                             void* kcache, void* vcache, int S, int past, int Smax, void* stream) {
   if (!c || !a || !w || !out || M <= 0 || N <= 0 || K <= 0 || (K % 8) || (block_n != 128 && block_n != 256))
-    return fail(VLY_ERR_INVALID, "vly_test_gemm: bad argument");
+    return fail(VLY_ERR_INVALID, "vly_test_gemm: bad argument (M %d, N %d, K %d, block_n %d)", M, N, K, block_n);
+  const bool norm = epi == EPI_LN_BIAS || epi == EPI_LN_BIAS_GELU || epi == EPI_RMS_QKV_ROPE || epi == EPI_RMS_SWIGLU || epi == EPI_RMS_F32;
+  if (norm && (!stats_in || stats_in_nt <= 0))
+    return fail(VLY_ERR_INVALID, "vly_test_gemm: epilogue %d needs stats_in and stats_in_nt > 0", epi);
   std::lock_guard<std::mutex> lk(c->mu);
   CK(cudaSetDevice(c->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const bf16 *A = (const bf16*)a, *W = (const bf16*)w;
   GemmParams p = {};
   p.M = M; p.N = N; p.K = K; p.out = out; p.ldo = N; p.bias = bias;
-  if (epi == EPI_BIAS) return launch_gemm<EPI_BIAS>(c, block_n, (const bf16*)a, K, (const bf16*)w, K, p, (cudaStream_t)stream);
-  if (epi == EPI_BIAS_RES_STATS) {
-    if (!residual || (N % 32)) return fail(VLY_ERR_INVALID, "vly_test_gemm: residual epilogue needs a residual and N %% 32 == 0");
-    p.residual = (const bf16*)residual; p.ldr = N;
-    return launch_gemm<EPI_BIAS_RES_STATS>(c, block_n, (const bf16*)a, K, (const bf16*)w, K, p, (cudaStream_t)stream);
+  p.stats_in = (const float2*)stats_in; p.stats_in_nt = stats_in_nt; p.inv_dim = 1.f / K; p.eps = eps;
+  switch (epi) {
+    case EPI_BIAS:
+      return launch_gemm<EPI_BIAS>(c, block_n, A, K, W, K, p, st);
+    case EPI_BIAS_RES_STATS:
+      if (!residual || (N % 32)) return fail(VLY_ERR_INVALID, "vly_test_gemm: the residual epilogue needs a residual and N %% 32 == 0");
+      p.residual = (const bf16*)residual; p.ldr = N; p.stats_out = (float2*)stats_out;
+      return launch_gemm<EPI_BIAS_RES_STATS>(c, block_n, A, K, W, K, p, st);
+    case EPI_LN_BIAS:
+    case EPI_LN_BIAS_GELU:
+      if (!colsum) return fail(VLY_ERR_INVALID, "vly_test_gemm: the LayerNorm epilogues need colsum");
+      p.colsum = colsum;
+      return epi == EPI_LN_BIAS ? launch_gemm<EPI_LN_BIAS>(c, block_n, A, K, W, K, p, st)
+                                : launch_gemm<EPI_LN_BIAS_GELU>(c, block_n, A, K, W, K, p, st);
+    case EPI_RMS_QKV_ROPE:
+      if (!kcache || !vcache || (N % 384) || S <= 0 || (M % S) || past < 0 || past + S > Smax || Smax > c->cfg.max_position_embeddings ||
+          !c->rope)
+        return fail(VLY_ERR_INVALID, "vly_test_gemm: the QKV epilogue needs K/V caches, N %% 384 == 0, M %% S == 0, "
+                    "past + S <= Smax <= max_position_embeddings and a RoPE table (S %d, past %d, Smax %d)", S, past, Smax);
+      p.ldo = N / 3; p.rope = c->rope; p.S = S; p.past = past; p.H = N / 3; p.nH = N / 384; p.Smax = Smax;
+      p.kcache = (bf16*)kcache; p.vcache = (bf16*)vcache;
+      return launch_gemm<EPI_RMS_QKV_ROPE>(c, block_n, A, K, W, K, p, st);
+    case EPI_RMS_SWIGLU:
+      if (N % 32) return fail(VLY_ERR_INVALID, "vly_test_gemm: the SwiGLU epilogue needs N %% 32 == 0");
+      p.ldo = N / 2;
+      return launch_gemm<EPI_RMS_SWIGLU>(c, block_n, A, K, W, K, p, st);
+    case EPI_RMS_F32:
+      return launch_gemm<EPI_RMS_F32>(c, block_n, A, K, W, K, p, st);
   }
   return fail(VLY_ERR_INVALID, "vly_test_gemm: unsupported epilogue %d", epi);
+}
+
+extern "C" int vly_test_prefill_attention(vly_ctx* c, const void* q, const void* kcache, const void* vcache, int B, int S, int past, int nH,
+                                          int Smax, const uint8_t* key_mask, void* out, void* stream) {
+  if (!c || !q || !kcache || !vcache || !out || B <= 0 || S <= 0 || past < 0 || nH <= 0 || Smax <= 0 || (Smax % 128) || past + S > Smax)
+    return fail(VLY_ERR_INVALID, "vly_test_prefill_attention: bad argument (B %d, S %d, past %d, heads %d, Smax %d)", B, S, past, nH, Smax);
+  std::lock_guard<std::mutex> lk(c->mu);
+  CK(cudaSetDevice(c->cfg.device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int words = Smax / 32;
+  uint32_t* key_bits = nullptr;
+  if (key_mask) {
+    TRY(ensure(c->w_tprefill, (size_t)B * words * 4));
+    key_bits = (uint32_t*)c->w_tprefill.p;
+    TRY(launch(c, pack_key_mask_kernel, {dim3(cdiv(words, 128), B), dim3(128), 0, st}, key_mask, past + S, words, key_bits));
+  }
+  return launch_prefill_attention(c, (const bf16*)q, (const bf16*)kcache, (const bf16*)vcache, Smax, key_bits, B, S, past, nH, (bf16*)out, st);
 }
 
 extern "C" int vly_test_vit_attention(vly_ctx* c, const void* qkv, int F, void* out, void* stream) {

@@ -63,9 +63,11 @@ struct GemmParams {
   long long peer_frame_off;
 };
 
-// x*sigmoid(1.702x) and x*sigmoid(x) on the fast MUFU path (ex2.approx + rcp.approx)
-// sigmoid(y) = 0.5 + 0.5 tanh(y / 2): ONE MUFU op (tanh.approx.f32, |rel err| ~ 2^-11, far below the bf16 rounding of the result)
-// instead of two (ex2 + rcp).  A 128 x 256 fc1 tile has 32768 activations per CTA: at 16 MUFU ops per clock per SM the
+// x*sigmoid(1.702x) and x*sigmoid(x) on the fast MUFU path
+// sigmoid(y) = 0.5 + 0.5 tanh(y / 2): ONE MUFU op (tanh.approx.f32) instead of two (ex2 + rcp).  tanh.approx has a relative
+// error of about 2^-11 (PTX ISA); the 0.5 + 0.5 tanh turns it into an ABSOLUTE error of ~2^-12 on sigmoid, so v * sigmoid(.) is
+// off by up to ~|v| 2^-12.  That is below the bf16 rounding of the result for v >~ 0 but exceeds it where the result is tiny:
+// quick-GELU arguments below about -1.6, SiLU arguments below about -2.7 (tests/test_gpu_prefill_per_op.py bounds it).  A 128 x 256 fc1 tile has 32768 activations per CTA: at 16 MUFU ops per clock per SM the
 // exp + reciprocal form alone took 4096 cycles -- the whole main loop of a K = 1024 tile.
 VLY_DEVINL float tanh_approx(float x) {
   float y;
